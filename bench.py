@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- TorchTrainer-shaped ResNet-50 DDP step (BASELINE.json configs[1]) on N B200s.
+"""bench.py -- TorchTrainer-shaped ResNet-50 DDP step (BASELINE.json configs[1]) on N H100s.
 
-    python bench.py --gpus 1 --steps 50 --warmup 5
+    python bench.py --gpus 1 --steps 50 --warmup 5 [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...   # the reference's CPU path (gloo DDP on host cores)
@@ -11,7 +11,10 @@ One step = forward + backward + Adam update of torchvision ResNet-50 (random ini
 224x224 batch, bf16 autocast, per-GPU batch 32 as in release/train_tests/benchmark/config.py:15),
 with the gradient synchronisation -- the hot path of this repository -- running in
 libb200_collective.so through the b200 c10d backend and the fused bf16 gradient hook.
-Rank 0 prints ONE JSON line (see DESIGN.md "Measurement").
+Rank 0 prints ONE JSON line (see DESIGN.md "Measurement").  With --dump-outputs DIR, rank 0
+also writes what the last timed step computed: the loss, and the same fixed, seeded sample of
+the all-reduced gradients and of the updated parameters (float32 .npy files, 32 MiB in all), so
+that two builds can be compared output for output on identical seeded inputs.
 """
 from __future__ import annotations
 
@@ -53,6 +56,8 @@ def parse_args():
     p.add_argument("--no-nccl-comparator", action="store_true", help="skip the in-line NCCL comparator leg (N>1)")
     p.add_argument("--profile", action="store_true",
                    help="under ncu: skip the end-to-end and sweep legs (numbers printed in this mode are not bench values)")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="write the last timed step's loss, gradients and parameters (seeded sample) as DIR/<name>.npy")
     p.add_argument("--cpu-worker", default=None, help=argparse.SUPPRESS)
     return p.parse_args()
 
@@ -70,7 +75,7 @@ def free_port():
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """Samples nvidia-smi during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi during the timed region (clocks, power and throttle reasons)."""
 
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -123,15 +128,38 @@ def build(device, seed=0):
     return model
 
 
-def train_step(model, opt, x, y, device_type):
+def train_step(model, opt, x, y, device_type, keep_grads=False):
     import torch
 
     with torch.autocast(device_type, dtype=torch.bfloat16):
         loss = torch.nn.functional.cross_entropy(model(x), y)
     loss.backward()
     opt.step()
-    opt.zero_grad(set_to_none=False)
+    if not keep_grads:  # the caller reads the synchronised gradients, then zeroes them
+        opt.zero_grad(set_to_none=False)
     return loss
+
+
+DUMP_SAMPLE = 1 << 22  # elements sampled from the flat gradient and parameter vectors
+
+
+def dump_outputs(out_dir, model, opt, loss):
+    """Writes the loss, and a fixed seeded sample of the flattened all-reduced gradients and
+    updated parameters (model.parameters() order), as float32 .npy files; then zeroes the
+    gradients the last step kept."""
+    import numpy as np
+    import torch
+
+    params = list(model.parameters())
+    flat_g = torch.cat([p.grad.detach().reshape(-1).float() for p in params])
+    flat_p = torch.cat([p.detach().reshape(-1).float() for p in params])
+    idx = np.sort(np.random.default_rng(0).choice(flat_p.numel(), min(DUMP_SAMPLE, flat_p.numel()), replace=False))
+    idx_t = torch.from_numpy(idx).to(flat_p.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().cpu().numpy().reshape(1))
+    np.save(os.path.join(out_dir, "grads_sample.npy"), flat_g.index_select(0, idx_t).cpu().numpy())
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat_p.index_select(0, idx_t).cpu().numpy())
+    opt.zero_grad(set_to_none=False)
 
 
 # ----------------------------------------------------------------------------- GPU arms
@@ -182,24 +210,28 @@ def run_gpu(args):
     dev_y = host_y.to(device)
     loss_host = torch.zeros((), dtype=torch.float32).pin_memory()
 
-    def timed(region_steps, resident: bool):
-        """Returns ms for `region_steps` steps (device time, this rank)."""
+    last = {}
+
+    def timed(region_steps, resident: bool, keep_last_grads=False):
+        """Returns ms for `region_steps` steps (device time, this rank).  With keep_last_grads the
+        last step leaves its synchronised gradients in place for dump_outputs()."""
         torch.cuda.synchronize()
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
         t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0.record()
-        for _ in range(region_steps):
+        for i in range(region_steps):
             if resident:
                 x, y = dev_x, dev_y
             else:
                 x = host_x.to(device, non_blocking=True)
                 y = host_y.to(device, non_blocking=True)
-            loss = train_step(model, opt, x, y, "cuda")
+            loss = train_step(model, opt, x, y, "cuda", keep_grads=keep_last_grads and i == region_steps - 1)
             if not resident:
                 loss_host.copy_(loss.detach().float(), non_blocking=True)
         t1.record()
+        last["loss"] = loss
         torch.cuda.synchronize()
         if world > 1:
             dist.barrier()
@@ -223,8 +255,9 @@ def run_gpu(args):
     if pg is not None:
         pg.timings = []
         pg.record_timings = True
+    dump = args.dump_outputs is not None
     with ClockSampler(local_rank) as clocks:
-        ms = max_over_ranks(timed(args.steps, resident=True))
+        ms = max_over_ranks(timed(args.steps, resident=True, keep_last_grads=dump and args.profile))
     if pg is not None:
         pg.record_timings = False
     launches = (pg.comm.launch_count - launches0) if (pg is not None and pg.comm is not None) else 0
@@ -244,7 +277,13 @@ def run_gpu(args):
     else:
         for _ in range(2):
             timed(1, resident=False)
-        ms_e2e = max_over_ranks(timed(args.steps, resident=False))
+        ms_e2e = max_over_ranks(timed(args.steps, resident=False, keep_last_grads=dump))
+    if dump:
+        if rank == 0:
+            dump_outputs(args.dump_outputs, model, opt, last["loss"])
+            log(f"outputs of the last timed step written to {args.dump_outputs}")
+        else:
+            opt.zero_grad(set_to_none=False)
 
     global_batch = B * world
     value = global_batch * args.steps / (ms / 1e3)
@@ -255,23 +294,8 @@ def run_gpu(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
-
-    def ncu_traffic():
-        """dram__bytes_read.sum + dram__bytes_write.sum per launch of grad_local_kernel from the
-        committed `ncu --set full` capture (profiles/r02/grad_local_kernel_ncu_full.csv)."""
-        try:
-            import csv
-
-            rows = list(csv.reader(open(os.path.join(ROOT, "profiles", "r02", "grad_local_kernel_ncu_full.csv"))))
-            hdr, units, data = rows[0], rows[1], rows[2:]
-            ri, wi = hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            tot = [float(d[ri]) * scale[units[ri]] + float(d[wi]) * scale[units[wi]] for d in data]
-            return sum(tot) / len(tot)
-        except Exception:
-            return None
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (3.35 TB/s HBM3, 700 W)"
 
     roofline = None
     if kernel_ms:
@@ -281,16 +305,16 @@ def run_gpu(args):
             # local stage of the gradient path: read fp32 + write fp32 per element
             alg = avg_elems * 8.0
             roofline = {"bound": "hbm", "achieved": alg / (avg_ms * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s",
-                        "traffic": ncu_traffic(), "kernel": "grad_local_kernel", "peak_source": peak_src,
-                        "note": "launches overlap the backward pass (separate stream); the ncu capture shows "
-                                "the fp32 write-back staying in the 126 MB L2",
+                        "traffic": None, "kernel": "grad_local_kernel", "peak_source": peak_src,
+                        "note": "launches overlap the backward pass (separate stream); a bucket that is "
+                                "still in the 50 MB L2 can beat the HBM bound",
                         "launch_ms": avg_ms, "algorithmic_bytes_per_launch": alg}
         else:
             wire_b = 2.0 if args.grad_wire == "bf16" else 4.0
             alg = avg_elems * wire_b * 2.0 * (world - 1) / world  # nccl-tests bus bytes
-            roofline = {"bound": "nvlink", "achieved": alg / (avg_ms * 1e-3) / 1e9, "peak": 900.0, "unit": "GB/s",
+            roofline = {"bound": "nvlink", "achieved": alg / (avg_ms * 1e-3) / 1e9, "peak": 450.0, "unit": "GB/s",
                         "traffic": None, "kernel": "grad_allreduce_kernel", "launch_ms": avg_ms,
-                        "peak_source": "nominal NVLink 5 per direction (measured peer copy 770 GB/s)",
+                        "peak_source": "H100 SXM data sheet: NVLink 4, 900 GB/s total = 450 GB/s per direction",
                         "algorithmic_bytes_per_launch": alg,
                         "note": "in-step launches include waiting for the slowest rank's bucket"}
         roofline["frac"] = roofline["achieved"] / roofline["peak"]
@@ -322,12 +346,12 @@ def run_gpu(args):
                        "grad_sync": ("b200 fused hook wire=" + args.grad_wire) if args.impl == "b200"
                        else "torch DDP + NCCL" + (" bf16_compress_hook" if args.grad_wire == "bf16" else ""),
                        "ddp_at_world_1": world == 1,
-                       "l2": "per-step activations+weights (>1 GB) exceed the 126 MB L2; no explicit flush"},
+                       "l2": "per-step activations+weights (>1 GB) exceed the 50 MB L2; no explicit flush"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int((host_x.numel() * 4 + host_y.numel() * 8) * world),
                     "d2h_bytes_per_step": 4 * world, "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": int(launches),
             "clocks": clocks.summary(),
-            "model_flops_frac": value * FLOPS_PER_SAMPLE / world / (float(peaks.get("bf16_tflops_sustained", 1411.0)) * 1e12),
+            "model_flops_frac": value * FLOPS_PER_SAMPLE / world / (float(peaks.get("bf16_tflops_sustained", 989.0)) * 1e12),
         }
         if roofline is not None:
             line["roofline"] = roofline

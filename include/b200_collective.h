@@ -1,7 +1,7 @@
 /*
  * b200_collective.h — C ABI of libb200_collective.so
  *
- * Blackwell-native (sm_100a) replacement for the device-side work that Ray's
+ * Hopper-native (H100, sm_90a) replacement for the device-side work that Ray's
  * GPU collective / tensor-transport hot path delegates to libnccl.  Every entry
  * point takes plain pointers, sizes and a raw cudaStream_t: no torch, cupy or
  * Ray types cross this boundary.  All functions return 0 on success or a
@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define B200_MAX_RANKS 8      /* one NVSwitch domain of a single HGX B200 host */
+#define B200_MAX_RANKS 8      /* one NVSwitch domain of a single HGX H100 host */
 #define B200_HANDLE_BYTES 256 /* size of the opaque bootstrap blob */
 
 typedef struct b200_comm *b200_comm_t;

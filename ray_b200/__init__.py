@@ -1,6 +1,6 @@
-"""ray_b200 -- Blackwell-native collectives and tensor transport behind Ray's plugin APIs.
+"""ray_b200 -- Hopper-native (H100) collectives and tensor transport behind Ray's plugin APIs.
 
-The device work lives in ``libb200_collective.so`` (hand-written sm_100a CUDA, C ABI in
+The device work lives in ``libb200_collective.so`` (hand-written sm_90a CUDA, C ABI in
 ``include/b200_collective.h``); this package is the host-side mirror of the reference
 interfaces for that path:
 

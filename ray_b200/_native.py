@@ -117,7 +117,7 @@ def load() -> ctypes.CDLL:
     if not path.exists():
         raise ImportError(
             f"{path} not found: build it with `python -m ray_b200.build` "
-            "(nvcc, sm_100a).  ray_b200 has no CPU fallback."
+            "(nvcc, sm_90a).  ray_b200 has no CPU fallback."
         )
     lib = ctypes.CDLL(str(path), mode=ctypes.RTLD_GLOBAL)
     for name, (restype, argtypes) in SIGNATURES.items():

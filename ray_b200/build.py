@@ -1,4 +1,4 @@
-"""Builds libb200_collective.so (sm_100a) in-tree with nvcc.
+"""Builds libb200_collective.so (sm_90a, H100) in-tree with nvcc.
 
     python -m ray_b200.build [--force] [--verbose]
 
@@ -26,7 +26,7 @@ SOURCES = ["bootstrap.cu", "allreduce.cu", "allreduce_pipe.cu", "reduce_ops.cu",
 HEADERS = ["common.cuh", "comm.h", "kernel_utils.cuh", "allreduce_core.cuh", "bulk_copy.cuh", "pipe.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--cudart", "static",
     "-Xcompiler", "-fPIC",
@@ -72,7 +72,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     nvcc = _nvcc()
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(len(SOURCES), os.cpu_count() or 4)) as ex:
         objs = list(ex.map(lambda s: _compile_one(nvcc, s, verbose), SOURCES))
-    cmd = [nvcc, "-shared", "--cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "--cudart", "static", "-gencode", "arch=compute_90a,code=sm_90a",
            "-o", str(LIB_PATH), *objs, "-lpthread", "-ldl", "-lrt"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -263,8 +263,8 @@ static bool nvls_capable(int dtype, int op) {
          (op == B200_SUM || op == B200_AVG);
 }
 
-// Measured on 2/4/8 B200s (profiles/r01): with two ranks the switch reduction saves no
-// traffic and the peer-load kernel is faster; from five ranks on NVLS wins at every size.
+// With two ranks the switch reduction saves no traffic and the peer-load kernel is faster; from
+// five ranks on NVLS wins at every size (tuned with one GPU per rank on an NVSwitch system).
 static bool nvls_pays_off(const b200_comm *c, size_t nbytes) {
   const long long min_world = c->params[B200_PARAM_NVLS_MIN_WORLD];
   if (min_world >= 0) return c->world >= min_world;
@@ -274,29 +274,27 @@ static bool nvls_pays_off(const b200_comm *c, size_t nbytes) {
 }
 
 // Zero-copy operands: the NVSwitch reduction saturates with far fewer CTAs than the GPU has SMs
-// (8 B200s, profiles/r01/tune_w8_v2_graph.log: 64 CTAs beat 100 and 148), so those launches are
-// capped at 64 CTAs.  Staged operands keep CTA-to-CTA barriers over the whole grid by default:
-// running their reduce phase on fewer CTAs (this parameter > 0) needs grid-wide waits, which
-// serialise the phases and measured slower (profiles/r01/sweep_w4_nvls_ctas.log).
+// (64 CTAs beat a whole-GPU grid), so those launches are capped at 64 CTAs.  Staged operands
+// keep CTA-to-CTA barriers over the whole grid by default: running their reduce phase on fewer
+// CTAs (this parameter > 0) needs grid-wide waits, which serialise the phases and are slower.
 static int nvls_ctas(const b200_comm *c) {
   const long long v = c->params[B200_PARAM_NVLS_CTAS];
   return v > 0 ? int(v) : 0;
 }
 
-// LL pays n-1 flag-doubled pushes per rank: measured break-even against the one-shot kernel is
-// ~32 KiB with 2 ranks and ~4 KiB with 8 (profiles/r01/final_w8_graph_sweeps.log).
+// LL pays n-1 flag-doubled pushes per rank: its break-even against the one-shot kernel is
+// ~32 KiB with 2 ranks and ~4 KiB with 8 (one GPU per rank, NVSwitch).
 static size_t ll_limit(const b200_comm *c) {
   const long long v = c->params[B200_PARAM_LL_MAX_BYTES];
   const size_t lim = v >= 0 ? size_t(v) : (size_t(64) << 10) / size_t(c->world) / (c->world > 4 ? 2 : 1);
   return lim < kLLMaxPayload ? lim : kLLMaxPayload;
 }
 
-// Measured break-even of the pipelined kernels against the phase-by-phase ones (profiles/r02).
+// Break-even of the pipelined kernels against the phase-by-phase ones (one GPU per rank, NVSwitch).
 static size_t pipe_min_bytes(const b200_comm *c) {
   const long long v = c->params[B200_PARAM_PIPE_MIN_BYTES];
   if (v >= 0) return size_t(v);
-  // 2 ranks: the pull kernel wins from 16 MiB (350 vs 330 GB/s; 64 MiB 519 vs 440, 1 GiB 619 vs 411);
-  // NVLS roles: from 128 MiB (8 ranks: 586 vs 559, 256 MiB 673 vs 611, 1 GiB 694 vs 627 GB/s)
+  // 2 ranks: the pull kernel wins from 16 MiB; NVLS roles from 128 MiB
   return c->world == 2 ? (size_t(16) << 20) : (size_t(128) << 20);
 }
 
@@ -308,11 +306,13 @@ static size_t oneshot_limit(const b200_comm *c) {
   if (c->params[B200_PARAM_ONESHOT_MAX_BYTES] >= 0) return size_t(c->params[B200_PARAM_ONESHOT_MAX_BYTES]);
   if (env >= 0) return size_t(env);
   // each rank reads world * nbytes in the one-shot scheme.  Break-even against the two-shot kernel
-  // (profiles/r01 sweeps: 2 ranks ~1 MiB, 8 ranks ~256 KiB; profiles/r02/bench_n4: 256 KiB one-shot
-  // 16 us, 1 MiB two-shot 24 us); the 0.5 MB PPO gradient vector of BASELINE configs[3] falls on
-  // the one-shot side at 2 and 4 ranks.
+  // is ~1 MiB with 2 ranks and ~256 KiB with 8; the 0.5 MB PPO gradient vector of BASELINE
+  // configs[3] falls on the one-shot side at 2 and 4 ranks.
   return (size_t(5) << 19) / size_t(c->world);  // 2.5 MiB / n
 }
+
+// a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
+const void *allreduce_module_anchor() { return reinterpret_cast<const void *>(&allreduce_ll_kernel<float, B200_SUM>); }
 
 }  // namespace b200
 

@@ -31,7 +31,7 @@ __device__ __forceinline__ void reduce_publish_rows(const DevComm &c, size_t off
   const int n = c.world, r = c.rank, t = threadIdx.x;
   if (G == 0) G = gridDim.x;  // CTAs [0, G) share the rows of this phase
   if (NVLS) {
-    constexpr int UNR = 4;  // 8 in flight measured slower on 8 GPUs (profiles/r01/tune_w8_v2_graph.log)
+    constexpr int UNR = 4;  // 8 in flight measured slower with 8 GPUs on one NVSwitch
     char *mc = c.mc_data + off;
     for (size_t row0 = blockIdx.x; row0 < g.R; row0 += G * UNR) {
       uint4 v[UNR];

@@ -112,7 +112,7 @@ __device__ __forceinline__ void mailbox_post(CopyMailbox *mb, uint32_t chunks_do
 // One thread: count this CTA's arrival on a chunk; the last arriver re-zeroes the counter and
 // returns true.  The caller has executed __threadfence_system() after the writes the arrival
 // stands for (one fence may cover a batch of arrivals: with bulk stores to a peer in flight a
-// system-scope fence costs ~4 us -- measured, profiles/r02/trace_push_v1.log), so by the time any
+// system-scope fence costs microseconds, see the in-kernel trace), so by the time any
 // CTA observes the final count every contribution has been performed system-wide, and the flag
 // stores that follow the observation are issued after it.
 __device__ __forceinline__ bool chunk_arrive_fenced(uint32_t *cnt, uint32_t expected) {
@@ -160,8 +160,8 @@ __device__ __forceinline__ int thread_wait_chunk(const DevComm &c, size_t flag_b
 }
 
 // Scout thread: the consumers of a chunk flag (copy-out, pull) must not pay for the flag wait in
-// their issue loop -- an ld.acquire.sys poll of n flags plus fence.proxy.async measured ~2 us per
-// chunk (profiles/r02/trace_pull_v1.log), more than the chunk's copy time.  A spare thread walks
+// their issue loop -- an ld.acquire.sys poll of n flags plus fence.proxy.async can cost more per
+// chunk than the chunk's copy time (in-kernel trace).  A spare thread walks
 // the chunks in order, does the acquiring waits and the proxy fence, and publishes its progress in
 // shared memory; the consumer's gate is then one shared-memory load.
 struct ChunkScout {
@@ -570,11 +570,10 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_push_kernel(DevComm c, 
 // ---------------------------------------------------------------------------
 // n == 2, pull: copy-in | pull-reduce
 //
-// Measured on B200 (profiles/r02/bulk_bench*.log): bulk LOADS from a peer reach 770 GB/s with 16
-// CTAs and complete on an mbarrier the moment the bytes are in shared memory, while bulk STORES
-// to a peer top out at 705 GB/s and are only known to be complete ~10 us later (wait_group) --
-// a lag the consumer of a push design has to sit out.  So each rank stages its tensor in its OWN
-// slot (local copy, cheap completion) and the PEER pulls it:
+// Bulk LOADS from a peer complete on an mbarrier the moment the bytes are in shared memory, while
+// bulk STORES to a peer are only known to be complete microseconds later (wait_group) -- a lag
+// the consumer of a push design has to sit out.  So each rank stages its tensor in its OWN slot
+// (local copy, cheap completion) and the PEER pulls it:
 //
 //   copy-in CTAs : user tensor -> own slot (bulk copies)                        -> flag0[k][rank]
 //   pull CTAs    : one thread keeps kPullLookahead bulk loads of the peer's slot in flight into a
@@ -715,7 +714,7 @@ __global__ void __launch_bounds__(kThreads + 32, 1) allreduce_pull_kernel(DevCom
 //                  the shared ring, bulk-store into the caller's output tensor for p.  The rank's
 //                  own tensor goes straight from the input to its output.  A scout thread per
 //                  pull CTA follows the peers' chunk flags.
-// NVLink carries only loads (775 GB/s measured, completion known exactly); nothing is staged twice.
+// NVLink carries only loads (completion known exactly); nothing is staged twice.
 // ---------------------------------------------------------------------------
 struct GatherOuts {
   char *p[kMaxRanks];
@@ -813,11 +812,12 @@ int set_dyn_smem(int device, const void *fn) {
   return B200_OK;
 }
 
-// Defaults measured on 2 / 4 / 8 B200s (profiles/r02/tune_n2.log, tune_n4.log, tune_n8.log):
+// Defaults (tuned on an NVSwitch system with one GPU per rank; not re-tuned on H100, where the
+// B200_PARAM_PIPE_* parameters override them):
 //   2 ranks (pull)      : 1 MiB chunks, 32 copy-in + 32 pull CTAs
 //   3-4 ranks (NVLS)    : 4 MiB chunks, 16 + 16 copy CTAs, 64 reduce CTAs
-//   5-8 ranks (NVLS)    : 8 MiB chunks, 16 + 16 copy CTAs, 32 reduce CTAs (more CTAs on the
-//                         switch reduction measured slower, as in round 1)
+//   5-8 ranks (NVLS)    : 8 MiB chunks, 16 + 16 copy CTAs, 32 reduce CTAs (the switch reduction
+//                         saturates with few CTAs)
 size_t pipe_chunk_bytes(const b200_comm *c) {
   const long long v = c->params[B200_PARAM_PIPE_CHUNK_BYTES];
   size_t C = v > 0 ? size_t(v) : (c->world == 2 ? (size_t(1) << 20) : (c->world <= 4 ? (size_t(4) << 20) : (size_t(8) << 20)));
@@ -1040,6 +1040,9 @@ int selftest_pipe_geometry(size_t nbytes, size_t chunk_bytes, int copy_ctas, int
   }
   return B200_OK;
 }
+
+// a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
+const void *allreduce_pipe_module_anchor() { return reinterpret_cast<const void *>(&allgather_pull_kernel); }
 
 }  // namespace b200
 

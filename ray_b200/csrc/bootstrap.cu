@@ -65,6 +65,10 @@ struct Driver {
   CUresult (*MulticastUnbind)(CUmemGenericAllocationHandle, CUdevice, size_t, size_t) = nullptr;
   CUresult (*MulticastGetGranularity)(size_t *, const CUmulticastObjectProp *,
                                       CUmulticastGranularity_flags) = nullptr;
+  CUresult (*FuncGetModule)(CUmodule *, CUfunction) = nullptr;
+  CUresult (*ModuleGetFunctionCount)(unsigned int *, CUmodule) = nullptr;
+  CUresult (*ModuleEnumerateFunctions)(CUfunction *, unsigned int, CUmodule) = nullptr;
+  CUresult (*FuncLoad)(CUfunction) = nullptr;
   bool ok = false;
   bool has_multicast = false;
 };
@@ -101,6 +105,10 @@ static Driver &driver() {
     ok &= load_sym("cuMemSetAccess", &d.MemSetAccess);
     ok &= load_sym("cuMemExportToShareableHandle", &d.MemExportToShareableHandle);
     ok &= load_sym("cuMemImportFromShareableHandle", &d.MemImportFromShareableHandle);
+    ok &= load_sym("cuFuncGetModule", &d.FuncGetModule);
+    ok &= load_sym("cuModuleGetFunctionCount", &d.ModuleGetFunctionCount);
+    ok &= load_sym("cuModuleEnumerateFunctions", &d.ModuleEnumerateFunctions);
+    ok &= load_sym("cuFuncLoad", &d.FuncLoad);
     d.ok = ok;
     bool mc = true;
     mc &= load_sym("cuMulticastCreate", &d.MulticastCreate);
@@ -394,6 +402,37 @@ static int map_handle(int device, CUmemGenericAllocationHandle h, size_t bytes, 
   return B200_OK;
 }
 
+// CUDA loads kernels lazily by default: the first launch of a kernel loads it, and loading may
+// wait for the kernels already running on the device.  A collective's kernels spin until their
+// peers' kernels arrive, so a load issued while one of them spins can hold back the very launch it
+// waits for -- ranks that share a GPU in one process then stall until the watchdog gives up (e.g.
+// the first reduce-scatter<f16, PROD> enqueued behind an LL all-reduce that waits for the peer).
+// Every kernel of the library is therefore loaded on a device before its first communicator
+// exists, i.e. before any kernel of the library can be waiting.
+static int preload_kernels(int device) {
+  static std::mutex mu;
+  static std::vector<int> loaded;
+  std::lock_guard<std::mutex> lk(mu);
+  for (int dev : loaded)
+    if (dev == device) return B200_OK;
+  Driver &d = driver();
+  const void *anchors[] = {allreduce_module_anchor(), allreduce_pipe_module_anchor(), copy_ops_module_anchor(),
+                           grad_module_anchor(),      p2p_module_anchor(),            reduce_ops_module_anchor()};
+  for (const void *anchor : anchors) {
+    cudaFunction_t f = nullptr;
+    B200_CHECK_CUDA(cudaGetFuncBySymbol(&f, anchor));
+    CUmodule mod = nullptr;
+    B200_CHECK_CU(d.FuncGetModule(&mod, reinterpret_cast<CUfunction>(f)));
+    unsigned int n = 0;
+    B200_CHECK_CU(d.ModuleGetFunctionCount(&n, mod));
+    std::vector<CUfunction> fns(n);
+    if (n) B200_CHECK_CU(d.ModuleEnumerateFunctions(fns.data(), n, mod));
+    for (CUfunction fn : fns) B200_CHECK_CU(d.FuncLoad(fn));
+  }
+  loaded.push_back(device);
+  return B200_OK;
+}
+
 static int region_create(b200_comm *c, Region *r, size_t bytes, size_t gran) {
   Driver &d = driver();
   r->bytes = round_up(bytes, gran);
@@ -524,9 +563,10 @@ int b200_comm_create(int world_size, int rank, int device, const b200_config_t *
   B200_CHECK_CUDA(cudaFree(nullptr));
   Driver &d = driver();
   if (!d.ok) {
-    set_error("CUDA driver lacks the virtual memory management API");
+    set_error("CUDA driver lacks the virtual memory management or module enumeration API (12.4+)");
     return B200_ERR_UNSUPPORTED;
   }
+  if (int rc = preload_kernels(device)) return rc;
 
   b200_comm *c = new b200_comm();
   c->world = world_size;
@@ -950,7 +990,7 @@ void b200_pool_free(void *ptr, size_t size, int device, void *stream) {
 }
 
 const char *b200_last_error(void) { return g_err; }
-const char *b200_version(void) { return "b200_collective 0.2 (sm_100a)"; }
+const char *b200_version(void) { return "b200_collective 0.2 (sm_90a)"; }
 
 size_t b200_dtype_size(int dtype) {
   switch (dtype) {

@@ -18,18 +18,18 @@
 namespace b200 {
 
 constexpr int kBulkTile = 32 << 10;  // bytes per tile
-constexpr int kBulkStages = 6;       // ring depth (6 x 32 KiB = 192 KiB of shared memory)
-// loads issued ahead of the store cursor -- measured with scripts/bulk_bench.cu (profiles/r02/
-// bulk_bench*.log): 3 is as good as anything for local HBM -> local HBM (49.6 GB/s per CTA) and
-// for local -> peer over NVLink (16 CTAs: 711 GB/s); waiting for completion with a lag of 2+
-// tiles costs nothing
+// ring depth: 6 x 32 KiB = 192 KiB of dynamic shared memory, within the H100's 227 KiB per block
+constexpr int kBulkStages = 6;
+// loads issued ahead of the store cursor (scripts/bulk_bench.cu sweeps it): 3 keeps the copy unit
+// busy for local HBM -> local HBM and for local -> peer over NVLink; waiting for completion with
+// a lag of 2+ tiles costs nothing
 constexpr int kBulkLookaheadLocal = 3;
 constexpr int kBulkLookaheadRemote = 3;
 // A ring buffer is free again as soon as its store has READ it (wait_group.read); the store's
-// global writes may still be in flight then.  Measured on B200 (profiles/r02): a bulk store to a
-// peer over NVLink takes ~6 us to COMPLETE, so bounding the stores in flight by the ring depth
-// (12 x 16 KiB in the first version) capped a CTA at 18 GB/s.  Completion is therefore tracked
-// separately and lazily: done(i) is reported once tile i + D has been issued (wait_group D).
+// global writes may still be in flight then.  A bulk store to a peer over NVLink takes
+// microseconds to COMPLETE, so bounding the stores in flight by the ring depth caps a CTA far
+// below the copy unit's rate.  Completion is therefore tracked separately and lazily: done(i) is
+// reported once tile i + D has been issued (wait_group D).
 constexpr int kBulkLagRemote = 4;  // completion lag D for stores that cross NVLink
 constexpr int kBulkLagLocal = 2;   // ... and for stores into local HBM
 // the two flavours of the engine
@@ -39,8 +39,8 @@ struct BulkLocal {
 struct BulkRemote {
   static constexpr int kLookahead = kBulkLookaheadRemote, kLag = kBulkLagRemote;
 };
-// source on a peer (bulk loads over NVLink), destination local: 5 loads in flight measured 703 GB/s
-// with 16 CTAs against 530 with 3 (profiles/r02/bulk_bench_pull.log)
+// source on a peer (bulk loads over NVLink), destination local: the longer peer latency wants
+// 5 loads in flight rather than 3
 struct BulkPull {
   static constexpr int kLookahead = 5, kLag = kBulkLagLocal;
 };
@@ -115,8 +115,8 @@ __device__ __forceinline__ BulkRing bulk_ring_init(char *dyn_smem) {
 // ---------------------------------------------------------------------------
 // Segment engine.  One thread issues every tile, and a single thread retires a dependent
 // instruction every ~5 cycles, so the per-tile instruction count IS the throughput limit
-// (measured: a first, index-based engine with two divisions and three lambda calls per tile
-// reached 30-36 GB/s per CTA where the bulk-copy unit does 50).  Here the work is a list of
+// (a first, index-based engine with two divisions and three lambda calls per tile left the
+// bulk-copy unit a third idle).  Here the work is a list of
 // SEGMENTS -- contiguous byte ranges [src, src+bytes) -> [dst, dst+bytes) -- and the tiles of a
 // segment are walked with pointer increments; the callbacks run once per segment, not per tile:
 //   seg(i)         -> BulkSeg of segment i (bytes > 0)

@@ -79,7 +79,7 @@ struct b200_comm {
   std::atomic<uint64_t> launches{0};
   int forced_blocks = 0;
   long long params[B200_PARAM_COUNT] = {-1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1};
-  int sm_count = 148;
+  int sm_count = 132;  // H100 SXM; replaced by cudaDeviceProp::multiProcessorCount at creation
   std::atomic<bool> aborted{false};
   std::mutex mu;
 
@@ -89,5 +89,12 @@ struct b200_comm {
 namespace b200 {
 // implemented in bootstrap.cu
 int check_usable(b200_comm *c);
+// one kernel of each translation unit (= CUDA module) of the library
+const void *allreduce_module_anchor();
+const void *allreduce_pipe_module_anchor();
+const void *copy_ops_module_anchor();
+const void *grad_module_anchor();
+const void *p2p_module_anchor();
+const void *reduce_ops_module_anchor();
 inline size_t round_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 }  // namespace b200

@@ -105,6 +105,9 @@ __global__ void barrier_kernel(DevComm c) {
   finish_launch(c);
 }
 
+// a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
+const void *copy_ops_module_anchor() { return reinterpret_cast<const void *>(&barrier_kernel); }
+
 }  // namespace b200
 
 using namespace b200;

@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(kThreads, 1) grad_allreduce_kernel(DevComm c, 
 constexpr int kLocalThreads = 256;
 // One thread = UNR x 16 bytes of the fp32 bucket (4 elements), whatever the wire type: nothing is
 // stored in wire format here, so the 8-element wire units of the multi-rank kernels would only
-// halve the thread count (ncu, 60 MB bucket: 20.0 us with 8-element units, 15.1 us with 4).
+// halve the thread count and leave too few bytes in flight.
 template <typename W>
 __device__ __forceinline__ uint4 wire_round_trip(uint4 v, float scale) {
   float f[4] = {__uint_as_float(v.x) * scale, __uint_as_float(v.y) * scale, __uint_as_float(v.z) * scale,
@@ -193,9 +193,9 @@ __global__ void grad_local_scalar_kernel(GradArgs a) {
 }
 
 template <typename W, int UNR>
-static void launch_grad_local(const GradArgs &a, cudaStream_t stream) {
+static void launch_grad_local(const GradArgs &a, int sm_count, cudaStream_t stream) {
   if (!is_aligned16(a.grad)) {
-    grad_local_scalar_kernel<W><<<1184, 256, 0, stream>>>(a);
+    grad_local_scalar_kernel<W><<<8 * sm_count, 256, 0, stream>>>(a);
     return;
   }
   const size_t U = a.count >> 2;
@@ -214,13 +214,13 @@ static int launch_grad(b200_comm *c, GradArgs a, cudaStream_t stream) {
   constexpr int E = Wire<W>::kElems;
   const size_t U = (a.count + E - 1) / E;
   if (c->world == 1) {
-    // units per thread: tuning knob, default measured on B200 (profiles/r02/grad_local_sweep.txt)
+    // units per thread: tuning knob (B200_PARAM_GRAD_LOCAL_UNROLL), 1 unless set
     const long long unr = c->params[B200_PARAM_GRAD_LOCAL_UNROLL];
     switch (unr > 0 ? int(unr) : 1) {
-      case 2: launch_grad_local<W, 2>(a, stream); break;
-      case 4: launch_grad_local<W, 4>(a, stream); break;
-      case 8: launch_grad_local<W, 8>(a, stream); break;
-      default: launch_grad_local<W, 1>(a, stream); break;
+      case 2: launch_grad_local<W, 2>(a, c->sm_count, stream); break;
+      case 4: launch_grad_local<W, 4>(a, c->sm_count, stream); break;
+      case 8: launch_grad_local<W, 8>(a, c->sm_count, stream); break;
+      default: launch_grad_local<W, 1>(a, c->sm_count, stream); break;
     }
     B200_LAUNCH_CHECK(c);
     return B200_OK;
@@ -235,6 +235,9 @@ static int launch_grad(b200_comm *c, GradArgs a, cudaStream_t stream) {
   B200_LAUNCH_CHECK(c);
   return B200_OK;
 }
+
+// a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
+const void *grad_module_anchor() { return reinterpret_cast<const void *>(&grad_local_scalar_kernel<float>); }
 
 }  // namespace b200
 

@@ -297,6 +297,9 @@ static int p2p_common(b200_comm *c, void *buf, size_t nbytes, int peer, cudaStre
   return B200_OK;
 }
 
+// a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
+const void *p2p_module_anchor() { return reinterpret_cast<const void *>(&get_bulk_kernel); }
+
 }  // namespace b200
 
 using namespace b200;

@@ -137,6 +137,9 @@ static int launch_reduce(b200_comm *c, const ReduceArgs &a, cudaStream_t stream)
   return B200_OK;
 }
 
+// a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
+const void *reduce_ops_module_anchor() { return reinterpret_cast<const void *>(&reducescatter_kernel<float, B200_SUM>); }
+
 }  // namespace b200
 
 using namespace b200;

@@ -1,5 +1,5 @@
 // bulk_bench.cu — per-SM throughput of cp.async.bulk copies (local HBM and peer over NVLink).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/bulk_bench scripts/bulk_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/bulk_bench scripts/bulk_bench.cu
 //   scripts/bulk_bench            (runs the whole matrix; needs 1 GPU, uses a 2nd one if present)
 #include <cstdio>
 #include <cstdlib>

@@ -6,7 +6,7 @@ allreduce : phase-by-phase kernels vs the chunk-pipelined ones (allreduce_pipe.c
             chunk size / copy CTAs / reduce CTAs, on ordinary tensors
 sendrecv  : ld/st p2p kernel vs the TMA bulk-copy kernel
 gradlocal : world-1 gradient kernel, units per thread (run with --world 1)
-Output: one line per measurement; the chosen defaults are recorded in profiles/r02/.
+Output: one line per measurement; the chosen defaults are the constants in ray_b200/csrc/.
 """
 import argparse
 import os
@@ -123,7 +123,7 @@ def gradlocal(g, args):
                 c = g.comms[0]
                 times = []
                 for _ in range(12):
-                    flush.zero_()  # evict the bucket from the 126 MB L2
+                    flush.zero_()  # evict the bucket from the L2 (50 MB on H100)
                     t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                     t0.record()
                     c.grad_allreduce(x, 0.5, wire)

@@ -1,7 +1,5 @@
 #!/bin/bash
-# Tuning pass on an N-GPU box (device-timed, CUDA-graph replayed).  The round-1 run of an earlier
-# version of this script (which also exercised the since-removed overlap experiments) is
-# profiles/r01/tune_w8_v2_graph.log.
+# Tuning pass on an N-GPU machine (device-timed, CUDA-graph replayed).
 set -x
 W=${1:-8}
 S="python scripts/bw_sweep.py --world $W"

@@ -57,7 +57,8 @@ class Workers:
             self.col.init_collective_group(self.n, r, backend="b200", group_name=group_name)
             if self.shared:
                 g = self.col.get_group_handle(group_name)
-                g.comm.set_blocks(max(1, 140 // self.n))
+                sms = torch.cuda.get_device_properties(self.devices[0]).multi_processor_count
+                g.comm.set_blocks(max(1, (sms - 8) // self.n))
 
         self.run(f)
 

@@ -57,7 +57,8 @@ class Actors:
         self.run(lambda r, c: c.initialize(r))
         if self.shared:
             for c in self.comms:
-                c.comm.set_blocks(max(1, 140 // n))
+                sms = torch.cuda.get_device_properties(self.devices[0]).multi_processor_count
+                c.comm.set_blocks(max(1, (sms - 8) // n))
 
     def run(self, fn):
         out, err = [None] * self.n, [None] * self.n
