@@ -186,6 +186,21 @@ int b200_barrier(b200_comm_t comm, void *stream);
 int b200_send(b200_comm_t comm, const void *buf, size_t nbytes, int peer, void *stream);
 int b200_recv(b200_comm_t comm, void *buf, size_t nbytes, int peer, void *stream);
 
+/* All-to-all(v).  ins[p] (send_counts[p] elements) goes to rank p; outs[p] (recv_counts[p]
+ * elements) receives what rank p passed as its ins[this rank].  ins, outs, send_counts and
+ * recv_counts are host arrays of world_size entries.  A zero count skips that direction of the
+ * pair, and its pointer may be NULL.  Pairwise contract, as for send/recv: send_counts[q] on rank
+ * p == recv_counts[p] on rank q.  No output may overlap an input (no in-place all-to-all), except
+ * that outs[this rank] may be ins[this rank] itself (then there is nothing to copy).
+ * One launch: every send and receive of this rank runs as a role of one grid on the
+ * point-to-point rings, so it interleaves in stream order with earlier and later b200_send /
+ * b200_recv on the same pairs (it does not stand in for a peer's concurrent b200_send /
+ * b200_recv); the own segment is copied in the same launch.  b200_comm_set_blocks must be the same
+ * on every rank; below 2 * (world_size - 1) CTAs every rank returns B200_ERR_INVALID.
+ * Counterpart of ProcessGroupNCCL's alltoall_base / alltoall (ncclSend / ncclRecv in a group). */
+int b200_alltoall(b200_comm_t comm, const void *const *ins, const size_t *send_counts,
+                  void *const *outs, const size_t *recv_counts, int dtype, void *stream);
+
 /* One-sided get (RDT's one-sided transport, experimental/rdt/cuda_ipc_transport.py:57-186, without
  * its same-GPU restriction): copies [src_heap_offset, +nbytes) of rank `src_rank`'s symmetric heap
  * into `dst` with a kernel that runs on THIS rank only.  The caller orders it after the owner's

@@ -90,6 +90,8 @@ SIGNATURES = {
     "b200_barrier": (c_int, [c_void_p, c_void_p]),
     "b200_send": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "b200_recv": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
+    "b200_alltoall": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_void_p), POINTER(c_size_t),
+                              c_int, c_void_p]),
     "b200_symm_base": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t)]),
     "b200_get": (c_int, [c_void_p, c_void_p, c_int, c_size_t, c_size_t, c_void_p]),
     "b200_grad_allreduce": (c_int, [c_void_p, c_void_p, c_size_t, c_float, c_int, c_void_p]),

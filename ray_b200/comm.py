@@ -295,6 +295,33 @@ class B200Comm:
     def barrier(self) -> None:
         N.check(self._lib.b200_barrier(self._h, self._stream()))
 
+    def alltoall(self, outs: Sequence[Optional[torch.Tensor]], ins: Sequence[Optional[torch.Tensor]]) -> None:
+        """All-to-all(v) in one launch: ``ins[p]`` goes to rank p, ``outs[p]`` receives rank p's
+        ``ins[this rank]``.  ``None`` means nothing moves in that direction with that peer; sizes
+        may differ per peer, but every rank must agree on the size of each pair's message."""
+        n = self.world_size
+        if len(outs) != n or len(ins) != n:
+            raise RuntimeError("The length of the tensor list operands to alltoall must be equal to world_size.")
+        in_ptrs, out_ptrs = (ctypes.c_void_p * n)(), (ctypes.c_void_p * n)()
+        send_counts, recv_counts = (ctypes.c_size_t * n)(), (ctypes.c_size_t * n)()
+        dtype = None
+        for tensors, ptrs, counts, what in ((ins, in_ptrs, send_counts, "input tensor"),
+                                           (outs, out_ptrs, recv_counts, "output tensor")):
+            for p, t in enumerate(tensors):
+                if t is None:
+                    continue
+                _check_cuda_contiguous(t, what)
+                if dtype is None:
+                    dtype = t.dtype
+                elif t.dtype != dtype:
+                    raise RuntimeError("All tensor operands to alltoall must have the same dtype.")
+                ptrs[p] = t.data_ptr()
+                counts[p] = t.numel()
+        if dtype is None:
+            return
+        N.check(self._lib.b200_alltoall(self._h, in_ptrs, send_counts, out_ptrs, recv_counts, dtype_code(dtype),
+                                        self._stream()))
+
     def send(self, tensor: torch.Tensor, peer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Enqueue a send on ``stream`` (default: the current stream of this rank's device)."""
         _check_cuda_contiguous(tensor)

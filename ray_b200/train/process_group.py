@@ -147,7 +147,6 @@ class B200ProcessGroup(dist.ProcessGroup):
         self._comm: Optional[B200Comm] = None
         self._device: Optional[torch.device] = None
         self._stream: Optional[torch.cuda.Stream] = None
-        self._stream2: Optional[torch.cuda.Stream] = None  # receive side of all-to-all style ops
         self._gloo = None
         self._lock = threading.Lock()
         #: when True every op appends (start_event, end_event, first_tensor_bytes, tag) to ``timings``;
@@ -184,7 +183,6 @@ class B200ProcessGroup(dist.ProcessGroup):
                 # are placed ahead of the queued compute CTAs as SMs free up
                 prio = torch.cuda.Stream.priority_range()[1] if hasattr(torch.cuda.Stream, "priority_range") else -1
                 self._stream = torch.cuda.Stream(device=self._device, priority=prio)
-                self._stream2 = torch.cuda.Stream(device=self._device, priority=prio)
             elif device.index is not None and device.index != self._device.index:
                 raise RuntimeError(f"b200 process group is bound to {self._device}, got a tensor on {device}")
             return self._comm
@@ -356,83 +354,66 @@ class B200ProcessGroup(dist.ProcessGroup):
         return self._run(tensors, fn, tensors)
 
     # ------------------------------------------------------------------ rooted / all-to-all ops
+    # gather, scatter and both all-to-all forms are one b200_alltoall launch each
     def gather(self, output_tensors, input_tensors, opts=None):
-        """Root receives every rank's tensor (c10d ``gather``): non-roots push to the root's inbox."""
+        """Root receives every rank's tensor (c10d ``gather``): an all-to-all in which every rank
+        sends only to the root."""
         if not self._all_cuda(input_tensors):
             return self._cpu_group().gather(output_tensors, input_tensors, opts)
         root = opts.rootRank if opts is not None else 0
 
         def fn(comm):
             for i, t in enumerate(input_tensors):
-                if self._rank == root:
-                    outs = output_tensors[i]
-                    for p in range(self._size):
-                        if p == root:
-                            outs[p].copy_(t)
-                        else:
-                            comm.recv(self._contig(outs[p]), p)
-                else:
-                    comm.send(self._contig(t), root)
+                ins = [None] * self._size
+                ins[root] = self._contig(t)
+                outs = [self._contig(o) for o in output_tensors[i]] if self._rank == root else [None] * self._size
+                comm.alltoall(outs, ins)
 
         flat = list(input_tensors) + [o for outs in output_tensors for o in outs]
         return self._run(flat, fn, output_tensors)
 
     def scatter(self, output_tensors, input_tensors, opts=None):
+        """Mirror image of ``gather``: the root sends ``input_tensors[i][p]`` to rank p."""
         if not self._all_cuda(output_tensors):
             return self._cpu_group().scatter(output_tensors, input_tensors, opts)
         root = opts.rootRank if opts is not None else 0
 
         def fn(comm):
             for i, out in enumerate(output_tensors):
-                if self._rank == root:
-                    ins = input_tensors[i]
-                    for p in range(self._size):
-                        if p == root:
-                            out.copy_(ins[p])
-                        else:
-                            comm.send(self._contig(ins[p]), p)
-                else:
-                    comm.recv(self._contig(out), root)
+                outs = [None] * self._size
+                outs[root] = self._contig(out)
+                ins = [self._contig(t) for t in input_tensors[i]] if self._rank == root else [None] * self._size
+                comm.alltoall(outs, ins)
 
         flat = list(output_tensors) + [t for ins in input_tensors for t in ins]
         return self._run(flat, fn, output_tensors)
-
-    def _exchange(self, comm, sends, recvs):
-        """Pairwise exchange: in step s this rank sends to rank+s and receives from rank-s.  Sends
-        go on the communication stream and receives on a second one, so a message larger than the
-        eager ring cannot deadlock two ranks that are both still sending."""
-        self._stream2.wait_stream(self._stream)
-        for step in range(1, self._size):
-            to, frm = (self._rank + step) % self._size, (self._rank - step) % self._size
-            if sends[to] is not None and sends[to].numel():
-                comm.send(sends[to], to, stream=self._stream)
-            if recvs[frm] is not None and recvs[frm].numel():
-                comm.recv(recvs[frm], frm, stream=self._stream2)
-        if recvs[self._rank] is not None and recvs[self._rank].numel():
-            recvs[self._rank].copy_(sends[self._rank])
-        self._stream.wait_stream(self._stream2)
 
     def alltoall_base(self, output, input, output_split_sizes, input_split_sizes, opts=None):  # noqa: A002
         if not input.is_cuda:
             return self._cpu_group().alltoall_base(output, input, output_split_sizes, input_split_sizes, opts)
 
-        def splits(t, sizes):
+        def splits(t, sizes, what):
             if not sizes:
                 if t.size(0) % self._size:
                     raise RuntimeError("alltoall_base: dim 0 must be divisible by the world size")
                 sizes = [t.size(0) // self._size] * self._size
-            return list(torch.split(t, list(sizes), dim=0))
+            sizes = list(sizes)
+            if len(sizes) != self._size:
+                raise RuntimeError(f"alltoall_base: {len(sizes)} {what} split sizes for world size {self._size}")
+            if sum(sizes) != t.size(0):
+                raise RuntimeError(f"alltoall_base: {what} split sizes sum to {sum(sizes)}, dim 0 is {t.size(0)}")
+            return list(torch.split(t, sizes, dim=0))
 
-        sends = [self._contig(x) for x in splits(input, input_split_sizes)]
-        recvs = [self._contig(x) for x in splits(output, output_split_sizes)]
-        return self._run([output, input], lambda comm: self._exchange(comm, sends, recvs), output)
+        sends = [self._contig(x) for x in splits(input, input_split_sizes, "input")]
+        recvs = [self._contig(x) for x in splits(output, output_split_sizes, "output")]
+        return self._run([output, input], lambda comm: comm.alltoall(recvs, sends), output)
 
     def alltoall(self, output_tensors, input_tensors, opts=None):
         if not self._all_cuda(input_tensors):
             return self._cpu_group().alltoall(output_tensors, input_tensors, opts)
         sends = [self._contig(t) for t in input_tensors]
         recvs = [self._contig(t) for t in output_tensors]
-        return self._run(list(output_tensors) + list(input_tensors), lambda comm: self._exchange(comm, sends, recvs),
+        return self._run(list(output_tensors) + list(input_tensors), lambda comm: comm.alltoall(recvs, sends),
                          output_tensors)
 
     # ------------------------------------------------------------------ fused gradient path

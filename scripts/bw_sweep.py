@@ -2,9 +2,15 @@
 GPU, launches replayed from CUDA graphs so host launch overhead does not pollute the numbers).
 
     python scripts/bw_sweep.py --world 2 [--algos oneshot,twoshot,nvls] [--blocks 0,32,64] \
-        [--min 1024 --max 1073741824] [--op allreduce|allgather|reducescatter|broadcast|sendrecv|grad]
+        [--min 1024 --max 1073741824] [--op allreduce|allgather|reducescatter|broadcast|sendrecv|grad|
+                                            alltoall|alltoall_p2p] [--split uniform|skew|local]
 
 Prints one line per (size, algo, blocks): us per launch, algbw, busbw (nccl-tests convention).
+--op takes a comma list; the ops then alternate at every size.  For the all-to-all ops the size
+is bytes per peer: ``alltoall`` is the one-launch b200_alltoall, ``alltoall_p2p`` the composition
+it replaces (n-1 sends on the rank's stream, n-1 receives on a second stream, a local copy).
+--split skew gives them MoE-like splits instead: rank r sends size >> k bytes to rank r+k (4:2:1:...,
+the own segment the largest); --split local keeps `size` bytes on the rank and sends 16 KiB to each peer.
 """
 import argparse
 import os
@@ -52,6 +58,37 @@ def time_graphs(g, make_call, iters, reps=3):
     return best
 
 
+def alltoall_operands(g, n, numel, dtype, split):
+    """ins[r][p] / outs[r][p] for every rank; returns them with the bytes one rank sends."""
+    es = torch.empty((), dtype=dtype).element_size()
+
+    def count(p, q):
+        if split == "skew":
+            return numel >> ((q - p) % n)
+        if split == "local":
+            return numel if p == q else min(numel, (16 << 10) // es)
+        return numel
+
+    counts = [[count(p, q) for q in range(n)] for p in range(n)]
+    ins = [[torch.ones(counts[r][p], dtype=dtype, device=g.device(r)) for p in range(n)] for r in range(n)]
+    outs = [[torch.empty(counts[p][r], dtype=dtype, device=g.device(r)) for p in range(n)] for r in range(n)]
+    return ins, outs, max(sum(row) for row in counts) * es
+
+
+def alltoall_p2p(c, r, n, outs, ins, side):
+    """The host composition the one-launch all-to-all replaces."""
+    cur = torch.cuda.current_stream()
+    side.wait_stream(cur)
+    for step in range(1, n):
+        to, frm = (r + step) % n, (r - step) % n
+        if ins[to].numel():
+            c.send(ins[to], to, stream=cur)
+        if outs[frm].numel():
+            c.recv(outs[frm], frm, stream=side)
+    outs[r].copy_(ins[r])
+    cur.wait_stream(side)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--world", type=int, default=2)
@@ -65,6 +102,8 @@ def main():
     ap.add_argument("--symm", action="store_true", help="operands in the symmetric heap (zero copy)")
     ap.add_argument("--nvls-min-world", type=int, default=-1)
     ap.add_argument("--nvls-ctas", default="-1", help="comma list of CTA counts for the NVLS reduce phase")
+    ap.add_argument("--split", default="uniform", choices=["uniform", "skew", "local"],
+                    help="all-to-all ops: bytes per peer (see above)")
     args = ap.parse_args()
     n = args.world
     dtype = getattr(torch, args.dtype)
@@ -74,6 +113,7 @@ def main():
           f"dtype={args.dtype} symm={args.symm}")
     for c in g.comms:
         c.set_param(N.PARAM_NVLS_MIN_WORLD, args.nvls_min_world)
+    side = [torch.cuda.Stream(device=d) for d in g.devices]  # receive stream of alltoall_p2p
     size = args.min
     es = torch.empty((), dtype=dtype).element_size()
     while size <= args.max:
@@ -93,42 +133,50 @@ def main():
                     continue
                 if algo == N.ALGO_LL and size > (64 << 10):
                     continue
-                if args.symm:
-                    for c in g.comms:
-                        c.symm_reset()
-                    xs = [g.comms[r].symm_empty((numel,), dtype) for r in range(n)]
-                    for x in xs:
-                        x.fill_(1)
-                else:
-                    xs = [torch.ones(numel, dtype=dtype, device=g.device(r)) for r in range(n)]
-                if args.op == "allreduce":
-                    call = lambda c, r: c.allreduce(xs[r], N.SUM, algo=algo)  # noqa: E731
-                    factor = 2 * (n - 1) / n
-                elif args.op == "grad":
-                    call = lambda c, r: c.grad_allreduce(xs[r], 1.0 / n, torch.bfloat16)  # noqa: E731
-                    factor = 2 * (n - 1) / n
-                elif args.op == "allgather":
-                    outs = [torch.empty(n * numel, dtype=dtype, device=g.device(r)) for r in range(n)]
-                    call = lambda c, r: c.allgather_into(outs[r], xs[r])  # noqa: E731
-                    factor = (n - 1)  # S_total = n*size; busbw = n*size/t*(n-1)/n
-                elif args.op == "reducescatter":
-                    ins = [torch.ones(n * numel, dtype=dtype, device=g.device(r)) for r in range(n)]
-                    call = lambda c, r: c.reducescatter_from(xs[r], ins[r], N.SUM)  # noqa: E731
-                    factor = (n - 1)
-                elif args.op == "broadcast":
-                    call = lambda c, r: c.broadcast(xs[r], 0)  # noqa: E731
-                    factor = 1.0
-                elif args.op == "sendrecv":
-                    call = lambda c, r: (c.send(xs[0], 1) if r == 0 else (c.recv(xs[1], 0) if r == 1 else None))  # noqa: E731
-                    factor = 1.0
-                else:
-                    raise SystemExit(f"unknown op {args.op}")
-                torch.cuda.synchronize()
-                us = time_graphs(g, call, iters)
-                algbw = size / us / 1e3
-                print(f"{args.op} {size:>11d} B  algo={aname:8s} blocks={blocks:3d} nvls_ctas={nctas:3d} {us:10.2f} us  "
-                      f"algbw={algbw:8.1f} GB/s  busbw={algbw * factor:8.1f} GB/s", flush=True)
-                del xs
+                for op in args.op.split(","):
+                    if args.symm:
+                        for c in g.comms:
+                            c.symm_reset()
+                        xs = [g.comms[r].symm_empty((numel,), dtype) for r in range(n)]
+                        for x in xs:
+                            x.fill_(1)
+                    else:
+                        xs = [torch.ones(numel, dtype=dtype, device=g.device(r)) for r in range(n)]
+                    if op == "allreduce":
+                        call = lambda c, r: c.allreduce(xs[r], N.SUM, algo=algo)  # noqa: E731
+                        factor = 2 * (n - 1) / n
+                    elif op == "grad":
+                        call = lambda c, r: c.grad_allreduce(xs[r], 1.0 / n, torch.bfloat16)  # noqa: E731
+                        factor = 2 * (n - 1) / n
+                    elif op == "allgather":
+                        outs = [torch.empty(n * numel, dtype=dtype, device=g.device(r)) for r in range(n)]
+                        call = lambda c, r: c.allgather_into(outs[r], xs[r])  # noqa: E731
+                        factor = (n - 1)  # S_total = n*size; busbw = n*size/t*(n-1)/n
+                    elif op == "reducescatter":
+                        ins = [torch.ones(n * numel, dtype=dtype, device=g.device(r)) for r in range(n)]
+                        call = lambda c, r: c.reducescatter_from(xs[r], ins[r], N.SUM)  # noqa: E731
+                        factor = (n - 1)
+                    elif op == "broadcast":
+                        call = lambda c, r: c.broadcast(xs[r], 0)  # noqa: E731
+                        factor = 1.0
+                    elif op == "sendrecv":
+                        call = lambda c, r: (c.send(xs[0], 1) if r == 0 else (c.recv(xs[1], 0) if r == 1 else None))  # noqa: E731
+                        factor = 1.0
+                    elif op in ("alltoall", "alltoall_p2p"):
+                        ins, outs, nbytes = alltoall_operands(g, n, numel, dtype, args.split)
+                        if op == "alltoall":
+                            call = lambda c, r: c.alltoall(outs[r], ins[r])  # noqa: E731
+                        else:
+                            call = lambda c, r: alltoall_p2p(c, r, n, outs[r], ins[r], side[r])  # noqa: E731
+                        factor = (n - 1) / n  # nccl-tests all-to-all: busbw = algbw * (n-1)/n
+                    else:
+                        raise SystemExit(f"unknown op {op}")
+                    torch.cuda.synchronize()
+                    us = time_graphs(g, call, iters)
+                    algbw = (nbytes if op.startswith("alltoall") else size) / us / 1e3
+                    print(f"{op} {size:>11d} B  algo={aname:8s} blocks={blocks:3d} nvls_ctas={nctas:3d} {us:10.2f} us  "
+                          f"algbw={algbw:8.1f} GB/s  busbw={algbw * factor:8.1f} GB/s", flush=True)
+                    del xs
         size *= args.step
     g.destroy()
 
