@@ -365,14 +365,11 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
   // the two staging passes with the NVLink phase (allreduce_pipe.cu).  They move whole 16-byte
   // units with the bulk-copy engine, so they need aligned operands.
   int pipe_variant = -1;
-  if (sym_off < 0 && is_aligned16(in) && is_aligned16(out) && (total & 15) == 0 && pipe_max_bytes(c, 0) > 0 &&
+  if (sym_off < 0 && is_aligned16(in) && is_aligned16(out) && (total & 15) == 0 && pipe_chunk_bytes(c) > 0 &&
       (algo == B200_ALGO_PIPE || (algo == B200_ALGO_AUTO && total >= pipe_min_bytes(c)))) {
     if (c->world == 2) pipe_variant = PIPE_PULL;
     else if (c->mc_active && nvls_capable(dtype, op)) pipe_variant = PIPE_NVLS;
     else if (algo == B200_ALGO_PIPE) pipe_variant = PIPE_PEER;  // AUTO without NVLS keeps the two-shot kernel
-    if (algo == B200_ALGO_PIPE && c->params[B200_PARAM_PIPE_VARIANT] >= 0)
-      pipe_variant = int(c->params[B200_PARAM_PIPE_VARIANT]);
-    if (pipe_variant == PIPE_NVLS && !(c->mc_active && nvls_capable(dtype, op))) pipe_variant = PIPE_PEER;
   } else if (algo == B200_ALGO_PIPE) {
     set_error("the pipelined all-reduce needs 16-byte aligned operands outside the symmetric heap "
               "and a size that is a multiple of 16 bytes");

@@ -4,11 +4,11 @@
 
 namespace b200 {
 
+// Which pipelined kernel runs: a function of (world, multicast, dtype, op), see b200_allreduce.
 enum PipeVariant {
-  PIPE_PUSH = 0,  // one-shot push into the peers' slots (kept for comparison; slower than PIPE_PULL)
-  PIPE_NVLS = 1,  // copy-in | multimem.ld_reduce + multimem.st | copy-out
-  PIPE_PEER = 2,  // copy-in | peer loads + peer stores         | copy-out
-  PIPE_PULL = 3   // n == 2: copy-in | bulk-load the peer's slot + reduce into the caller's tensor
+  PIPE_NVLS,  // n >= 3: copy-in | multimem.ld_reduce + multimem.st | copy-out
+  PIPE_PEER,  // n >= 3: copy-in | peer loads + peer stores         | copy-out
+  PIPE_PULL   // n == 2: copy-in | bulk-load the peer's slot + reduce into the caller's tensor
 };
 
 // chunk size C of the pipeline (B200_PARAM_PIPE_CHUNK_BYTES, default 1 MiB)

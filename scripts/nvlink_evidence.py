@@ -4,12 +4,10 @@ For every collective kernel of the library: device time per launch (CUDA events 
 launches, max over ranks), the nccl-tests bus bandwidth, and the NVLink bytes that actually crossed
 the links of GPU 0 during the loop, read from the driver's NVLink counters through NVML
 (NVML_FI_DEV_NVLINK_THROUGHPUT_DATA_TX / _RX, KiB, all links; RAW = including protocol overhead).
-This is the multi-GPU counterpart of an ncu capture: ncu serialises kernels, and the kernels of a
-collective wait for each other across GPUs, so they cannot be replayed one at a time.
+A profiler that replays kernels one at a time cannot measure these: the kernels of a collective
+wait for each other across GPUs.
 
-    python scripts/nvlink_evidence.py --world 2 [--ncu-range CASE]   # CASE: run one case inside
-                                                                      # cudaProfilerStart/Stop for
-                                                                      # ncu --replay-mode app-range
+    python scripts/nvlink_evidence.py --world 2 [--out FILE.json]
 """
 import argparse
 import json
@@ -27,7 +25,6 @@ from ray_b200.testing import LocalGroup
 MiB = 1 << 20
 ap = argparse.ArgumentParser()
 ap.add_argument("--world", type=int, default=2)
-ap.add_argument("--ncu-range", default=None)
 ap.add_argument("--out", default=None)
 args = ap.parse_args()
 n = args.world
@@ -58,12 +55,12 @@ def nvlink_kib():
 
 
 def cases():
-    def ar(size, algo, variant=-1, dtype=torch.float32):
+    def ar(size, algo, dtype=torch.float32):
         xs = [torch.ones(size // torch.empty((), dtype=dtype).element_size(), dtype=dtype, device=g.device(r)) for r in range(n)]
 
         def call(c, r):
             c.allreduce(xs[r], N.SUM, algo=algo)
-        return call, size, 2 * (n - 1) / n, dict(variant=variant)
+        return call, size, 2 * (n - 1) / n
 
     yield "allreduce_ll_kernel 4KiB", ar(4096, N.ALGO_LL)
     yield "allreduce_oneshot_kernel 256KiB", ar(256 << 10, N.ALGO_ONESHOT)
@@ -71,55 +68,43 @@ def cases():
     if g.has_multicast:
         yield "allreduce_twoshot_kernel<NVLS> 64MiB", ar(64 * MiB, N.ALGO_NVLS)
     if n == 2:
-        yield "allreduce_pull_kernel 64MiB", ar(64 * MiB, N.ALGO_PIPE, 3)
-        yield "allreduce_pull_kernel 256MiB", ar(256 * MiB, N.ALGO_PIPE, 3)
-        yield "allreduce_push_kernel 64MiB", ar(64 * MiB, N.ALGO_PIPE, 0)
+        yield "allreduce_pull_kernel 64MiB", ar(64 * MiB, N.ALGO_PIPE)
+        yield "allreduce_pull_kernel 256MiB", ar(256 * MiB, N.ALGO_PIPE)
     else:
         if g.has_multicast:
-            yield "allreduce_pipe_kernel<NVLS> 256MiB", ar(256 * MiB, N.ALGO_PIPE, 1)
-        yield "allreduce_pipe_kernel<peer> 64MiB", ar(64 * MiB, N.ALGO_PIPE, 2)
+            yield "allreduce_pipe_kernel<NVLS> 256MiB", ar(256 * MiB, N.ALGO_PIPE)
+        # int32 has no NVLS reduction, so it takes the peer ld/st roles even with multicast
+        yield "allreduce_pipe_kernel<peer> 64MiB int32", ar(64 * MiB, N.ALGO_PIPE, torch.int32)
     per = 64 * MiB // n // 4
     xs = [torch.ones(per, device=g.device(r)) for r in range(n)]
     ys = [torch.empty(per * n, device=g.device(r)) for r in range(n)]
-    yield "allgather_pull_kernel 64MiB total", ((lambda c, r: c.allgather_into(ys[r], xs[r])), per * 4 * n, (n - 1) / n, {})
+    yield "allgather_pull_kernel 64MiB total", ((lambda c, r: c.allgather_into(ys[r], xs[r])), per * 4 * n, (n - 1) / n)
     small = [torch.ones(64 << 10, device=g.device(r)) for r in range(n)]
     smo = [torch.empty((64 << 10) * n, device=g.device(r)) for r in range(n)]
-    yield "allgather_kernel 256KiB/rank", ((lambda c, r: c.allgather_into(smo[r], small[r])), (256 << 10) * n, (n - 1) / n, {})
+    yield "allgather_kernel 256KiB/rank", ((lambda c, r: c.allgather_into(smo[r], small[r])), (256 << 10) * n, (n - 1) / n)
     ins = [torch.ones(per * n, device=g.device(r)) for r in range(n)]
     outs = [torch.empty(per, device=g.device(r)) for r in range(n)]
-    yield "reducescatter_kernel 64MiB total", ((lambda c, r: c.reducescatter_from(outs[r], ins[r], N.SUM)), per * 4 * n, (n - 1) / n, {})
+    yield "reducescatter_kernel 64MiB total", ((lambda c, r: c.reducescatter_from(outs[r], ins[r], N.SUM)), per * 4 * n, (n - 1) / n)
     b = [torch.ones(64 * MiB // 4, device=g.device(r)) for r in range(n)]
-    yield "broadcast_kernel 64MiB", ((lambda c, r: c.broadcast(b[r], 0)), 64 * MiB, 1.0, {})
+    yield "broadcast_kernel 64MiB", ((lambda c, r: c.broadcast(b[r], 0)), 64 * MiB, 1.0)
     red = [torch.ones(16 * MiB // 4, device=g.device(r)) for r in range(n)]
-    yield "reduce_kernel 16MiB", ((lambda c, r: c.reduce(red[r], 0, N.SUM)), 16 * MiB, 1.0, {})
+    yield "reduce_kernel 16MiB", ((lambda c, r: c.reduce(red[r], 0, N.SUM)), 16 * MiB, 1.0)
     p2p = [torch.ones(64 * MiB // 4, device=g.device(r)) for r in range(n)]
-    yield "p2p_bulk_kernel send+recv 64MiB", ((lambda c, r: c.send(p2p[0], 1) if r == 0 else (c.recv(p2p[1], 0) if r == 1 else None)), 64 * MiB, 1.0, {})
+    yield "p2p_bulk_kernel send+recv 64MiB", ((lambda c, r: c.send(p2p[0], 1) if r == 0 else (c.recv(p2p[1], 0) if r == 1 else None)), 64 * MiB, 1.0)
     sm = [torch.ones(4096 // 4, device=g.device(r)) for r in range(n)]
-    yield "p2p_kernel send+recv 4KiB", ((lambda c, r: c.send(sm[0], 1) if r == 0 else (c.recv(sm[1], 0) if r == 1 else None)), 4096, 1.0, {})
+    yield "p2p_kernel send+recv 4KiB", ((lambda c, r: c.send(sm[0], 1) if r == 0 else (c.recv(sm[1], 0) if r == 1 else None)), 4096, 1.0)
     gr = [torch.ones(25 * MiB // 4, device=g.device(r)) for r in range(n)]
-    yield "grad_allreduce_kernel 25MiB fp32 bucket, bf16 wire", ((lambda c, r: c.grad_allreduce(gr[r], 1.0 / n, torch.bfloat16)), 25 * MiB // 2, 2 * (n - 1) / n, {})
+    yield "grad_allreduce_kernel 25MiB fp32 bucket, bf16 wire", ((lambda c, r: c.grad_allreduce(gr[r], 1.0 / n, torch.bfloat16)), 25 * MiB // 2, 2 * (n - 1) / n)
     dst = torch.empty(64 * MiB, dtype=torch.uint8, device=g.device(1 % n))
-    yield "get_bulk_kernel (one-sided) 64MiB", ((lambda c, r: c.get(dst, 0, 0) if r == 1 % n else None), 64 * MiB, 1.0, {})
-    yield "barrier_kernel", ((lambda c, r: c.barrier()), 0, 0.0, {})
+    yield "get_bulk_kernel (one-sided) 64MiB", ((lambda c, r: c.get(dst, 0, 0) if r == 1 % n else None), 64 * MiB, 1.0)
+    yield "barrier_kernel", ((lambda c, r: c.barrier()), 0, 0.0)
 
 
 rows = []
-for name, (call, size, factor, opt) in cases():
-    if args.ncu_range and args.ncu_range not in name:
-        continue
-    for c in g.comms:
-        c.set_param(N.PARAM_PIPE_VARIANT, opt.get("variant", -1))
+for name, (call, size, factor) in cases():
     iters = 200 if size <= MiB else (30 if size <= 64 * MiB else 10)
     for _ in range(3):
         g.run(call)
-    if args.ncu_range:
-        torch.cuda.synchronize()
-        torch.cuda.profiler.start()
-        g.run(call)
-        torch.cuda.synchronize()
-        torch.cuda.profiler.stop()
-        print("ncu range done:", name)
-        continue
     torch.cuda.synchronize()
     k0 = nvlink_kib()
     starts, ends = [], []
@@ -149,8 +134,6 @@ for name, (call, size, factor, opt) in cases():
            "frac_of_900": round(max(tx or 0, rx or 0) / us / 1e3 / 900, 3) if (tx or rx) else None}
     rows.append(row)
     print(json.dumps(row), flush=True)
-for c in g.comms:
-    c.set_param(N.PARAM_PIPE_VARIANT, -1)
 if args.out and rows:
     json.dump(rows, open(args.out, "w"), indent=1)
 g.destroy()

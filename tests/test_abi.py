@@ -24,6 +24,23 @@ def test_header_declares_what_the_binding_binds():
     assert sorted(_native.SIGNATURES) == declared
 
 
+def _declared_enum(name):
+    text = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    body = re.search(r"typedef enum \{([^}]*)\}\s*" + name + r"\s*;", text).group(1)
+    return {k[len("B200_"):]: int(v) for k, v in re.findall(r"(B200_\w+)\s*=\s*(-?\d+)", body)}
+
+
+def test_header_enums_match_the_binding_constants():
+    for enum, prefix in (("b200_status_t", ("OK", "ERR_")), ("b200_algo_t", ("ALGO_",)),
+                         ("b200_param_t", ("PARAM_",))):
+        declared = _declared_enum(enum)
+        count = declared.pop("PARAM_COUNT", None)
+        bound = {k: v for k, v in vars(_native).items() if k.startswith(prefix) and isinstance(v, int)}
+        assert declared == bound, enum
+        if count is not None:
+            assert sorted(declared.values()) == list(range(count))
+
+
 def test_library_exports_every_declared_symbol(native_lib):
     out = subprocess.run(["nm", "-D", "--defined-only", str(_native.LIB_PATH)], capture_output=True, text=True,
                          check=True).stdout

@@ -1,8 +1,8 @@
 """GPU parity tests of the chunk-pipelined all-reduce kernels (allreduce_pipe.cu: TMA bulk-copy
 roles + reduce role synchronised by per-chunk flags) against the rank-ascending oracle.
 
-Peer ld/st and push variants are bit exact against the oracle for every dtype; the NVLS variant
-(multi-GPU boxes only) is exact on integer-valued data and within 1e-6 * sum|x| otherwise.
+The pull (2 ranks) and peer ld/st kernels are bit exact against the oracle for every dtype; the
+NVLS kernel (multi-GPU boxes only) is exact on integer-valued data and within 1e-6 * sum|x| otherwise.
 """
 import numpy as np
 import pytest
@@ -24,25 +24,15 @@ def pipe_groups(native_lib):
 
     cache = {}
 
-    def get(n):
-        if n not in cache:
-            cache[n] = LocalGroup(n, timeout_ms=20000, staging_bytes=40 << 20, inbox_bytes=2 << 20)
-        return cache[n]
+    def get(n, multicast=True):
+        if (n, multicast) not in cache:
+            cache[n, multicast] = LocalGroup(n, timeout_ms=20000, staging_bytes=40 << 20, inbox_bytes=2 << 20,
+                                             enable_multicast=multicast)
+        return cache[n, multicast]
 
     yield get
     for g in cache.values():
         g.destroy()
-
-
-def _variants(g, world):
-    from ray_b200 import _native as N
-
-    out = [("peer", 2)]
-    if world == 2:
-        out += [("pull", 3), ("push", 0)]
-    if g.has_multicast:
-        out.append(("nvls", 1))
-    return out, N
 
 
 def _rand(numel, dtype, seed):
@@ -62,41 +52,43 @@ def _np(t):
 
 @pytest.mark.parametrize("world", [2, 3, 4, 8])
 def test_pipelined_allreduce_matches_oracle(pipe_groups, world):
+    """Each pipelined kernel through the inputs that select it: pull at world 2; at world >= 3 NVLS
+    where the multicast mapping exists and the dtype / op allow it, peer ld/st otherwise.  A case
+    that takes NVLS also runs on a group created without multicast, where it takes peer ld/st."""
+    from ray_b200 import _native as N
+
     g = pipe_groups(world)
-    variants, N = _variants(g, world)
     cases = [(torch.float32, N.SUM), (torch.int32, N.SUM), (torch.bfloat16, N.SUM), (torch.float64, N.MAX),
              (torch.uint8, N.SUM), (torch.float32, N.AVG)]
-    for vname, vcode in variants:
-        for c in g.comms:
-            c.set_param(N.PARAM_PIPE_VARIANT, vcode)
-        try:
-            for dtype, op in cases:
-                if vname == "nvls" and not (dtype in (torch.float32, torch.bfloat16) and op in (N.SUM, N.AVG)):
-                    continue
-                es = torch.empty((), dtype=dtype).element_size()
-                for nbytes in SIZES:
-                    numel = nbytes // es
-                    host = [_rand(numel, dtype, 1000 * world + 17 * r + nbytes % 97) for r in range(world)]
-                    if vname == "nvls":  # integer-valued: any summation order is exact
-                        host = [(h.float() * 4).round().clamp(-64, 64).to(dtype) for h in host]
-                    xs = [h.to(g.device(r)) for r, h in enumerate(host)]
-                    g.run(lambda c, r: c.allreduce(xs[r], op, algo=N.ALGO_PIPE))
-                    half = dtype in (torch.bfloat16, torch.float16)
-                    want = O.reduce_rank_ascending([_np(h) for h in host], op,
-                                                   accumulate="fp32" if half else "native")
-                    for r in range(world):
-                        got = _np(xs[r])
-                        if vname == "nvls":
-                            # the switch may return +0.0 where IEEE gives -0.0 (observed): compare values
-                            assert np.array_equal(got.astype(np.float64), np.asarray(want).astype(np.float64)), \
-                                (vname, world, dtype, op, nbytes, r)
-                            assert np.array_equal(got.view(np.uint8), _np(xs[0]).view(np.uint8))  # replicas agree
-                        else:
-                            assert np.array_equal(got.view(np.uint8), np.asarray(want).view(np.uint8)), \
-                                (vname, world, dtype, op, nbytes, r)
-        finally:
-            for c in g.comms:
-                c.set_param(N.PARAM_PIPE_VARIANT, -1)
+    for dtype, op in cases:
+        if world == 2:
+            kernels = [("pull", g)]
+        elif g.has_multicast and dtype in (torch.float32, torch.bfloat16) and op in (N.SUM, N.AVG):
+            kernels = [("nvls", g), ("peer", pipe_groups(world, multicast=False))]
+        else:
+            kernels = [("peer", g)]
+        for kname, grp in kernels:
+            es = torch.empty((), dtype=dtype).element_size()
+            for nbytes in SIZES:
+                numel = nbytes // es
+                host = [_rand(numel, dtype, 1000 * world + 17 * r + nbytes % 97) for r in range(world)]
+                if kname == "nvls":  # integer-valued: any summation order is exact
+                    host = [(h.float() * 4).round().clamp(-64, 64).to(dtype) for h in host]
+                xs = [h.to(grp.device(r)) for r, h in enumerate(host)]
+                grp.run(lambda c, r: c.allreduce(xs[r], op, algo=N.ALGO_PIPE))
+                half = dtype in (torch.bfloat16, torch.float16)
+                want = O.reduce_rank_ascending([_np(h) for h in host], op,
+                                               accumulate="fp32" if half else "native")
+                for r in range(world):
+                    got = _np(xs[r])
+                    if kname == "nvls":
+                        # the switch may return +0.0 where IEEE gives -0.0 (observed): compare values
+                        assert np.array_equal(got.astype(np.float64), np.asarray(want).astype(np.float64)), \
+                            (kname, world, dtype, op, nbytes, r)
+                        assert np.array_equal(got.view(np.uint8), _np(xs[0]).view(np.uint8))  # replicas agree
+                    else:
+                        assert np.array_equal(got.view(np.uint8), np.asarray(want).view(np.uint8)), \
+                            (kname, world, dtype, op, nbytes, r)
 
 
 @pytest.mark.parametrize("world", [2, 4])
@@ -164,6 +156,9 @@ def test_pipeline_tuning_parameters_do_not_change_results(pipe_groups, world):
     numel = (4 * MiB + 16 * 5) // 4
     host = [_rand(numel, torch.float32, 77 + r) for r in range(world)]
     want = O.reduce_rank_ascending([h.numpy() for h in host], N.SUM)
+    with pytest.raises(N.B200Error) as err:
+        g.comms[0].set_param(10, 0)  # B200_PARAM_COUNT: one past the last parameter
+    assert err.value.status == N.ERR_INVALID
     try:
         for chunk, copy_ctas, red_ctas in ((1 * MiB, 1, 2), (2 * MiB, 2, 3), (1 * MiB, 4, 1), (3 * MiB, 2, 5)):
             for c in g.comms:
@@ -290,8 +285,9 @@ def test_pull_allgather_is_byte_exact(pipe_groups, world):
 @pytest.mark.parametrize("world", [3, 4])
 def test_chunk_ring_handles_messages_larger_than_the_staging_slot_in_one_launch(pipe_groups, world):
     """n >= 3 pipeline with the slot used as a ring of chunks: a message several times the slot
-    size goes through ONE launch (copy-in of chunk k waits for the copy-out of chunk k - R);
-    B200_PARAM_PIPE_RING=0 splits it into several launches and must give the same bits."""
+    size goes through ONE launch (copy-in of chunk k waits for the copy-out of chunk k - R).  A
+    chunk the slot holds fewer than 4 times leaves the ring off: the message is then split into
+    launches of whole chunks that fit the slot, and must give the same bits."""
     from ray_b200 import _native as N
 
     g = pipe_groups(world)  # 40 MiB staging slot
@@ -299,20 +295,18 @@ def test_chunk_ring_handles_messages_larger_than_the_staging_slot_in_one_launch(
     host = [(torch.arange(numel, dtype=torch.float32) % 1021) * (r + 1) - 3 * r for r in range(world)]
     want = sum(host)
     try:
-        for chunk in (1 * MiB, 4 * MiB):
-            for ring in (-1, 0):
-                for c in g.comms:
-                    c.set_param(N.PARAM_PIPE_CHUNK_BYTES, chunk)
-                    c.set_param(N.PARAM_PIPE_RING, ring)
-                xs = [h.to(g.device(r)) for r, h in enumerate(host)]
-                before = g.comms[0].launch_count
-                g.run(lambda c, r: c.allreduce(xs[r], N.SUM, algo=N.ALGO_PIPE))
-                launches = g.comms[0].launch_count - before
-                assert launches == (1 if ring == -1 else 3), (chunk, ring, launches)
-                for r in range(world):
-                    assert torch.equal(xs[r].cpu(), want), (world, chunk, ring, r)
-                del xs
+        # 12 MiB chunks: 3 fit the slot, so no ring; 36 MiB per launch
+        for chunk, expect in ((1 * MiB, 1), (4 * MiB, 1), (12 * MiB, 3)):
+            for c in g.comms:
+                c.set_param(N.PARAM_PIPE_CHUNK_BYTES, chunk)
+            xs = [h.to(g.device(r)) for r, h in enumerate(host)]
+            before = g.comms[0].launch_count
+            g.run(lambda c, r: c.allreduce(xs[r], N.SUM, algo=N.ALGO_PIPE))
+            launches = g.comms[0].launch_count - before
+            assert launches == expect, (chunk, launches)
+            for r in range(world):
+                assert torch.equal(xs[r].cpu(), want), (world, chunk, r)
+            del xs
     finally:
         for c in g.comms:
             c.set_param(N.PARAM_PIPE_CHUNK_BYTES, -1)
-            c.set_param(N.PARAM_PIPE_RING, -1)
