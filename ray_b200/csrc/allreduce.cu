@@ -19,7 +19,7 @@
 // CTA b's of all ranks (flags in the signal pad) is the only synchronisation needed:
 // no grid-wide sync, no host involvement.
 #include "allreduce_core.cuh"
-#include "pipe.h"
+#include "policy.h"
 
 namespace b200 {
 
@@ -219,8 +219,6 @@ allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-static int nvls_ctas(const b200_comm *c);
-static size_t ll_limit(const b200_comm *c);
 template <typename T, int OP>
 static int launch_allreduce(b200_comm *c, const char *in, char *out, size_t nbytes, int algo,
                             long long sym_off, cudaStream_t stream) {
@@ -258,59 +256,6 @@ static int launch_allreduce(b200_comm *c, const char *in, char *out, size_t nbyt
   return B200_OK;
 }
 
-static bool nvls_capable(int dtype, int op) {
-  return (dtype == B200_F32 || dtype == B200_F16 || dtype == B200_BF16) &&
-         (op == B200_SUM || op == B200_AVG);
-}
-
-// With two ranks the switch reduction saves no traffic and the peer-load kernel is faster; from
-// five ranks on NVLS wins at every size (tuned with one GPU per rank on an NVSwitch system).
-static bool nvls_pays_off(const b200_comm *c, size_t nbytes) {
-  const long long min_world = c->params[B200_PARAM_NVLS_MIN_WORLD];
-  if (min_world >= 0) return c->world >= min_world;
-  if (c->world <= 2) return false;
-  if (c->world <= 4) return nbytes >= (size_t(128) << 20);
-  return true;
-}
-
-// Zero-copy operands: the NVSwitch reduction saturates with far fewer CTAs than the GPU has SMs
-// (64 CTAs beat a whole-GPU grid), so those launches are capped at 64 CTAs.  Staged operands
-// keep CTA-to-CTA barriers over the whole grid by default: running their reduce phase on fewer
-// CTAs (this parameter > 0) needs grid-wide waits, which serialise the phases and are slower.
-static int nvls_ctas(const b200_comm *c) {
-  const long long v = c->params[B200_PARAM_NVLS_CTAS];
-  return v > 0 ? int(v) : 0;
-}
-
-// LL pays n-1 flag-doubled pushes per rank: its break-even against the one-shot kernel is
-// ~32 KiB with 2 ranks and ~4 KiB with 8 (one GPU per rank, NVSwitch).
-static size_t ll_limit(const b200_comm *c) {
-  const long long v = c->params[B200_PARAM_LL_MAX_BYTES];
-  const size_t lim = v >= 0 ? size_t(v) : (size_t(64) << 10) / size_t(c->world) / (c->world > 4 ? 2 : 1);
-  return lim < kLLMaxPayload ? lim : kLLMaxPayload;
-}
-
-// Break-even of the pipelined kernels against the phase-by-phase ones (one GPU per rank, NVSwitch).
-static size_t pipe_min_bytes(const b200_comm *c) {
-  const long long v = c->params[B200_PARAM_PIPE_MIN_BYTES];
-  if (v >= 0) return size_t(v);
-  // 2 ranks: the pull kernel wins from 16 MiB; NVLS roles from 128 MiB
-  return c->world == 2 ? (size_t(16) << 20) : (size_t(128) << 20);
-}
-
-static size_t oneshot_limit(const b200_comm *c) {
-  static long long env = [] {
-    const char *s = getenv("B200_ONESHOT_MAX_BYTES");
-    return s ? atoll(s) : -1ll;
-  }();
-  if (c->params[B200_PARAM_ONESHOT_MAX_BYTES] >= 0) return size_t(c->params[B200_PARAM_ONESHOT_MAX_BYTES]);
-  if (env >= 0) return size_t(env);
-  // each rank reads world * nbytes in the one-shot scheme.  Break-even against the two-shot kernel
-  // is ~1 MiB with 2 ranks and ~256 KiB with 8; the 0.5 MB PPO gradient vector of BASELINE
-  // configs[3] falls on the one-shot side at 2 and 4 ranks.
-  return (size_t(5) << 19) / size_t(c->world);  // 2.5 MiB / n
-}
-
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
 const void *allreduce_module_anchor() { return reinterpret_cast<const void *>(&allreduce_ll_kernel<float, B200_SUM>); }
 
@@ -320,22 +265,11 @@ using namespace b200;
 
 extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t count, int dtype,
                               int op, int algo, void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
-  if (op < 0 || op >= B200_OP_COUNT) {
-    set_error("unsupported reduce op %d", op);
-    return B200_ERR_UNSUPPORTED;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op))) return rc;
   if (count == 0) return B200_OK;
-  if (!in || !out) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!in || !out) return null_tensor_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   const size_t total = count * es;
@@ -365,7 +299,7 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
   // the two staging passes with the NVLink phase (allreduce_pipe.cu).  They move whole 16-byte
   // units with the bulk-copy engine, so they need aligned operands.
   int pipe_variant = -1;
-  if (sym_off < 0 && is_aligned16(in) && is_aligned16(out) && (total & 15) == 0 && pipe_chunk_bytes(c) > 0 &&
+  if (sym_off < 0 && is_aligned16(in) && is_aligned16(out) && (total & 15) == 0 && pipe_fits(c) &&
       (algo == B200_ALGO_PIPE || (algo == B200_ALGO_AUTO && total >= pipe_min_bytes(c)))) {
     if (c->world == 2) pipe_variant = PIPE_PULL;
     else if (c->mc_active && nvls_capable(dtype, op)) pipe_variant = PIPE_NVLS;
@@ -377,15 +311,12 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
   }
 
   // Messages larger than one staging slot are processed slot by slot.
-  const size_t chunk_max = sym_off >= 0 ? total : (pipe_variant >= 0 ? pipe_max_bytes(c, pipe_variant) : c->staging_bytes);
-  for (size_t done = 0; done < total;) {
-    const size_t nbytes = (total - done) < chunk_max ? (total - done) : chunk_max;
-    if (pipe_variant >= 0 && (algo == B200_ALGO_PIPE || nbytes >= pipe_min_bytes(c) || nbytes > c->staging_bytes)) {
-      rc = launch_allreduce_pipe_dyn(c, src + done, dst + done, nbytes, dtype, op, pipe_variant, stream);
-      if (rc) return rc;
-      done += nbytes;
-      continue;
-    }
+  const size_t step = sym_off >= 0         ? total
+                      : pipe_variant >= 0 ? pipe_plan(c, PipeVariant(pipe_variant)).max_bytes
+                                          : c->staging_bytes;
+  return for_each_piece(total, step, [&](size_t done, size_t nbytes) -> int {
+    if (pipe_variant >= 0 && (algo == B200_ALGO_PIPE || nbytes >= pipe_min_bytes(c) || nbytes > c->staging_bytes))
+      return launch_allreduce_pipe_dyn(c, src + done, dst + done, nbytes, dtype, op, pipe_variant, stream);
     int a = algo;
     if (a == B200_ALGO_AUTO || a == B200_ALGO_PIPE) {
       if (nbytes <= ll_limit(c)) a = B200_ALGO_LL;
@@ -396,15 +327,13 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
     if (a == B200_ALGO_LL && nbytes > kLLMaxPayload) a = B200_ALGO_ONESHOT;
     if (a == B200_ALGO_ONESHOT && nbytes > c->staging_bytes) a = B200_ALGO_TWOSHOT;
     const long long so = sym_off >= 0 ? sym_off + (long long)done : -1;
+    int rc2 = B200_OK;
     B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, {
-                          rc = launch_allreduce<T, OP>(c, src + done, dst + done, nbytes, a, so, stream);
+                          rc2 = launch_allreduce<T, OP>(c, src + done, dst + done, nbytes, a, so, stream);
                         }));
-    if (rc) return rc;
-    done += nbytes;
-  }
-  return B200_OK;
+    return rc2;
+  });
 }
-
 
 // ---- multi-tensor entry ------------------------------------------------------------
 namespace b200 {
@@ -432,17 +361,9 @@ static int launch_multi(b200_comm *c, const TensorTable &tb, cudaStream_t stream
 // dtypes take one fused launch per tensor.
 extern "C" int b200_allreduce_multi(b200_comm_t c, void *const *ptrs, const size_t *counts,
                                     int ntensors, int dtype, int op, void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
-  if (op < 0 || op >= B200_OP_COUNT) {
-    set_error("unsupported reduce op %d", op);
-    return B200_ERR_UNSUPPORTED;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op))) return rc;
   if (ntensors < 0 || (ntensors > 0 && (!ptrs || !counts))) {
     set_error("invalid tensor list");
     return B200_ERR_INVALID;

@@ -31,7 +31,7 @@
 // every rank's completion of a launch depends on every peer having started that launch.
 #include "allreduce_core.cuh"
 #include "bulk_copy.cuh"
-#include "pipe.h"
+#include "policy.h"
 
 #include <algorithm>
 #include <utility>
@@ -662,12 +662,6 @@ __global__ void __launch_bounds__(kThreads, 1) allgather_pull_kernel(DevComm c, 
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-static int pow2_floor(int x) {
-  int p = 1;
-  while (p * 2 <= x) p *= 2;
-  return p;
-}
-
 // Opt the kernel into kBulkSmemBytes of dynamic shared memory, once per (device, kernel): the
 // attribute call is kept out of the steady-state launch path (and out of stream capture).
 int set_dyn_smem(int device, const void *fn) {
@@ -681,60 +675,16 @@ int set_dyn_smem(int device, const void *fn) {
   return B200_OK;
 }
 
-// Defaults (tuned on an NVSwitch system with one GPU per rank; not re-tuned on H100, where the
-// B200_PARAM_PIPE_* parameters override them):
-//   2 ranks (pull)      : 1 MiB chunks, 32 copy-in + 32 pull CTAs
-//   3-4 ranks (NVLS)    : 4 MiB chunks, 16 + 16 copy CTAs, 64 reduce CTAs
-//   5-8 ranks (NVLS)    : 8 MiB chunks, 16 + 16 copy CTAs, 32 reduce CTAs (the switch reduction
-//                         saturates with few CTAs)
-size_t pipe_chunk_bytes(const b200_comm *c) {
-  const long long v = c->params[B200_PARAM_PIPE_CHUNK_BYTES];
-  size_t C = v > 0 ? size_t(v) : (c->world == 2 ? (size_t(1) << 20) : (c->world <= 4 ? (size_t(4) << 20) : (size_t(8) << 20)));
-  const size_t quantum = size_t(32) * kBulkTile;  // C / G is a whole number of tiles for any power-of-two G <= 32
-  C = round_up(C, quantum);
-  const size_t fit = c->staging_bytes / quantum * quantum;  // a chunk must fit the staging slot
-  return C < fit ? C : fit;                                 // 0: slot too small for the pipeline
-}
-
-// chunk ring of the n >= 3 pipeline: on whenever the slot holds at least 4 chunks
-static bool pipe_ring_enabled(const b200_comm *c, int variant) {
-  if (variant != PIPE_NVLS && variant != PIPE_PEER) return false;  // pull kernels: the READER is a peer
-  const size_t C = pipe_chunk_bytes(c);
-  return C && c->staging_bytes / C >= 4;
-}
-
-size_t pipe_max_bytes(const b200_comm *c, int variant) {
-  const size_t C = pipe_chunk_bytes(c);
-  if (C == 0) return 0;
-  size_t cap = pipe_ring_enabled(c, variant) ? ~size_t(0) : c->staging_bytes;
-  const size_t by_chunks = size_t(kMaxPipeChunks) * C;
-  cap = cap < by_chunks ? cap : by_chunks;
-  return cap / C * C;  // whole chunks, so a split message continues on a chunk boundary
-}
-
 template <typename T, int OP>
 int launch_allreduce_pipe(b200_comm *c, const char *in, char *out, size_t nbytes, int variant,
                           cudaStream_t stream) {
-  PipeArgs a{in, out, nbytes, c->staging_bytes, pipe_chunk_bytes(c), 0, 0};
-  if (pipe_ring_enabled(c, variant) && nbytes > c->staging_bytes / a.chunk_bytes * a.chunk_bytes)
-    a.ring_chunks = uint32_t(c->staging_bytes / a.chunk_bytes);
-  const long long pc = c->params[B200_PARAM_PIPE_COPY_CTAS];
-  const long long pr = c->params[B200_PARAM_PIPE_RED_CTAS];
-  int G = pc > 0 ? int(pc) : (variant == PIPE_PULL ? 32 : 16);
-  int Gr = pr > 0 ? int(pr) : (variant == PIPE_PULL ? 32 : (c->world <= 4 ? 64 : 32));
-  const int roles = variant == PIPE_PULL ? 1 : 2;  // copy roles: copy-in (+ copy-out for n >= 3)
-  int cap = c->forced_blocks > 0 ? c->forced_blocks : c->sm_count;
-  if (roles * G + Gr > cap) {  // shared-GPU harness / small parts: shrink, keep at least one reducer
-    while (G > 1 && roles * G + 1 > cap / 2) G /= 2;
-    Gr = cap - roles * G;
-    if (Gr < 1) {
-      set_error("pipelined all-reduce needs at least %d CTAs (have %d)", roles + 1, cap);
-      return B200_ERR_UNSUPPORTED;
-    }
+  const PipePlan p = pipe_plan(c, PipeVariant(variant));
+  if (p.work_ctas < 1) {
+    set_error("pipelined all-reduce needs at least %d CTAs (have %d)", variant == PIPE_PULL ? 2 : 3, grid_cap(c));
+    return B200_ERR_UNSUPPORTED;
   }
-  G = pow2_floor(G > 32 ? 32 : G);
-  a.copy_ctas = G;
-  const int grid = roles * G + Gr;
+  const uint32_t ring = nbytes > size_t(p.ring) * p.chunk ? p.ring : 0;
+  PipeArgs a{in, out, nbytes, c->staging_bytes, p.chunk, p.copy_ctas, ring};
   DevComm dc = c->dev();
   int rc = B200_OK;
   if (variant == PIPE_PULL) {
@@ -744,12 +694,12 @@ int launch_allreduce_pipe(b200_comm *c, const char *in, char *out, size_t nbytes
     }
     auto k = allreduce_pull_kernel<T, OP>;
     if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(k)))) return rc;
-    k<<<grid, kThreads + 32, kBulkSmemBytes, stream>>>(dc, a);  // + one service warp (scout)
+    k<<<p.grid, kThreads + 32, kBulkSmemBytes, stream>>>(dc, a);  // + one service warp (scout)
   } else if (variant == PIPE_NVLS) {
     if constexpr (Multimem<T>::kSum && (OP == B200_SUM || OP == B200_AVG)) {
       auto k = allreduce_pipe_kernel<T, OP, true>;
       if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(k)))) return rc;
-      k<<<grid, kThreads + 32, kBulkSmemBytes, stream>>>(dc, a);  // + one service warp
+      k<<<p.grid, kThreads + 32, kBulkSmemBytes, stream>>>(dc, a);  // + one service warp
     } else {
       set_error("NVLS all-reduce supports SUM/AVG on f32/f16/bf16 only");
       return B200_ERR_UNSUPPORTED;
@@ -757,7 +707,7 @@ int launch_allreduce_pipe(b200_comm *c, const char *in, char *out, size_t nbytes
   } else {
     auto k = allreduce_pipe_kernel<T, OP, false>;
     if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(k)))) return rc;
-    k<<<grid, kThreads + 32, kBulkSmemBytes, stream>>>(dc, a);  // + one service warp
+    k<<<p.grid, kThreads + 32, kBulkSmemBytes, stream>>>(dc, a);  // + one service warp
   }
   B200_LAUNCH_CHECK(c);
   return B200_OK;
@@ -772,32 +722,19 @@ int launch_allreduce_pipe_dyn(b200_comm *c, const char *in, char *out, size_t nb
   return rc;
 }
 
-// in / outs[p] 16-byte aligned, nbytes a multiple of 16 and <= pipe_max_bytes()
+// in / outs[p] 16-byte aligned, nbytes a multiple of 16 and <= pipe_plan(c, PIPE_GATHER).max_bytes
 int launch_allgather_pull(b200_comm *c, const char *in, char *const *outs, size_t nbytes, cudaStream_t stream) {
-  PipeArgs a{in, nullptr, nbytes, c->staging_bytes, pipe_chunk_bytes(c), 0, 0};
-  if (c->params[B200_PARAM_PIPE_CHUNK_BYTES] <= 0) a.chunk_bytes = round_up(size_t(1) << 20, size_t(32) * kBulkTile);
-  const long long pc = c->params[B200_PARAM_PIPE_COPY_CTAS];
-  const long long pr = c->params[B200_PARAM_PIPE_RED_CTAS];
-  int G = pc > 0 ? int(pc) : 16;
-  // pull CTAs also move the rank's own tensor (in -> out): half of all bytes at 2 ranks, 1/8 at 8
-  int Gp = pr > 0 ? int(pr) : (c->world == 2 ? 64 : (c->world <= 4 ? 48 : 32));
-  int cap = c->forced_blocks > 0 ? c->forced_blocks : c->sm_count;
-  if (G + Gp > cap) {
-    while (G > 1 && G + 1 > cap / 2) G /= 2;
-    Gp = cap - G;
-    if (Gp < 1) {
-      set_error("pull all-gather needs at least 2 CTAs (have %d)", cap);
-      return B200_ERR_UNSUPPORTED;
-    }
+  const PipePlan p = pipe_plan(c, PIPE_GATHER);
+  if (p.work_ctas < 1) {
+    set_error("pull all-gather needs at least 2 CTAs (have %d)", grid_cap(c));
+    return B200_ERR_UNSUPPORTED;
   }
-  G = pow2_floor(G > 32 ? 32 : G);
-  a.copy_ctas = G;
-  if (a.chunk_bytes > c->staging_bytes) a.chunk_bytes = c->staging_bytes / (size_t(32) * kBulkTile) * (size_t(32) * kBulkTile);
+  PipeArgs a{in, nullptr, nbytes, c->staging_bytes, p.chunk, p.copy_ctas, 0};
   GatherOuts o{};
-  for (int p = 0; p < c->world; ++p) o.p[p] = outs[p];
+  for (int q = 0; q < c->world; ++q) o.p[q] = outs[q];
   int rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(allgather_pull_kernel));
   if (rc) return rc;
-  allgather_pull_kernel<<<G + Gp, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a, o);
+  allgather_pull_kernel<<<p.grid, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a, o);
   B200_LAUNCH_CHECK(c);
   return B200_OK;
 }

@@ -1,8 +1,7 @@
 // copy_ops.cu — all-gather (SURVEY K2 with the K6 un-flatten copies fused away),
 // broadcast (K4) and the flag-only barrier (K7).  These kernels move bytes; they do
 // not depend on the element type.
-#include "kernel_utils.cuh"
-#include "pipe.h"
+#include "policy.h"
 
 namespace b200 {
 
@@ -114,18 +113,11 @@ using namespace b200;
 
 extern "C" int b200_allgather(b200_comm_t c, const void *in, void *const *outs, size_t count,
                               int dtype, void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es))) return rc;
   if (count == 0) return B200_OK;
-  if (!in || !outs) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!in || !outs) return null_tensor_error();
   for (int p = 0; p < c->world; ++p)
     if (!outs[p]) {
       set_error("output tensor %d is null", p);
@@ -139,30 +131,17 @@ extern "C" int b200_allgather(b200_comm_t c, const void *in, void *const *outs, 
     return B200_OK;
   }
   // Large aligned operands: the pull kernel (TMA copy-in + bulk loads of the peers' slots straight
-  // into the caller's output tensors, allreduce_pipe.cu).  B200_PARAM_AG_PULL_MIN_BYTES = per-rank
-  // size from which it is used (default 4 MiB; 0 = never).
-  {
-    const long long pm = c->params[B200_PARAM_AG_PULL_MIN_BYTES];
-    const size_t pull_min = pm >= 0 ? size_t(pm) : (size_t(4) << 20);  // 4 ranks: 1 MiB/rank 49 us pulled vs 28 us staged
-    bool aligned = is_aligned16(in) && (total & 15) == 0 && pm != 0 && pipe_chunk_bytes(c) > 0;
-    for (int p = 0; p < c->world; ++p) aligned = aligned && is_aligned16(outs[p]);
-    if (aligned && total >= pull_min) {
-      // a pull kernel: no chunk ring, so one launch takes at most one staging slot
-      const size_t cap = pipe_max_bytes(c, PIPE_PULL) / (size_t(1) << 20) * (size_t(1) << 20);
-      const size_t step = cap ? cap : c->staging_bytes;
-      for (size_t done = 0; done < total;) {
-        const size_t nbytes = (total - done) < step ? (total - done) : step;
-        char *o[kMaxRanks] = {};
-        for (int p = 0; p < c->world; ++p) o[p] = static_cast<char *>(outs[p]) + done;
-        rc = launch_allgather_pull(c, static_cast<const char *>(in) + done, o, nbytes, stream);
-        if (rc) return rc;
-        done += nbytes;
-      }
-      return B200_OK;
-    }
+  // into the caller's output tensors, allreduce_pipe.cu).
+  bool aligned = is_aligned16(in) && (total & 15) == 0 && pipe_fits(c);
+  for (int p = 0; p < c->world; ++p) aligned = aligned && is_aligned16(outs[p]);
+  if (aligned && ag_pull_pays_off(c, total)) {
+    return for_each_piece(total, pipe_plan(c, PIPE_GATHER).max_bytes, [&](size_t done, size_t nbytes) {
+      char *o[kMaxRanks] = {};
+      for (int p = 0; p < c->world; ++p) o[p] = static_cast<char *>(outs[p]) + done;
+      return launch_allgather_pull(c, static_cast<const char *>(in) + done, o, nbytes, stream);
+    });
   }
-  for (size_t done = 0; done < total;) {
-    const size_t nbytes = (total - done) < c->staging_bytes ? (total - done) : c->staging_bytes;
+  return for_each_piece(total, c->staging_bytes, [&](size_t done, size_t nbytes) -> int {
     AGArgs a{};
     a.in = static_cast<const char *>(in) + done;
     for (int p = 0; p < c->world; ++p) a.outs[p] = static_cast<char *>(outs[p]) + done;
@@ -172,45 +151,28 @@ extern "C" int b200_allgather(b200_comm_t c, const void *in, void *const *outs, 
     int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
     allgather_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
     B200_LAUNCH_CHECK(c);
-    done += nbytes;
-  }
-  return B200_OK;
+    return B200_OK;
+  });
 }
 
 extern "C" int b200_broadcast(b200_comm_t c, void *buf, size_t count, int dtype, int root,
                               void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
-  if (root < 0 || root >= c->world) {
-    set_error("root rank %d out of range for world size %d", root, c->world);
-    return B200_ERR_INVALID;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_rank(c, root, "root"))) return rc;
   if (count == 0 || c->world == 1) return B200_OK;
-  if (!buf) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!buf) return null_tensor_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
-  const size_t total = count * es;
-  for (size_t done = 0; done < total;) {
-    const size_t nbytes = (total - done) < c->staging_bytes ? (total - done) : c->staging_bytes;
+  return for_each_piece(count * es, c->staging_bytes, [&](size_t done, size_t nbytes) -> int {
     BcastArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
     const size_t U = make_units(nbytes).total();
     int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
-    // The multicast store pays off once more than one peer would pull from the root.
-    const bool nvls = c->mc_active && c->world > 2 && nbytes >= (size_t(64) << 10);
-    if (nvls) broadcast_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
+    if (broadcast_nvls(c, nbytes)) broadcast_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
     else broadcast_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
     B200_LAUNCH_CHECK(c);
-    done += nbytes;
-  }
-  return B200_OK;
+    return B200_OK;
+  });
 }
 
 extern "C" int b200_barrier(b200_comm_t c, void *stream_) {

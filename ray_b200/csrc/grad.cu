@@ -13,6 +13,7 @@
 #include <type_traits>
 
 #include "allreduce_core.cuh"
+#include "policy.h"
 
 namespace b200 {
 
@@ -209,8 +210,7 @@ static int launch_grad(b200_comm *c, GradArgs a, cudaStream_t stream) {
   }
   const size_t rows = (U + size_t(c->world) * kThreads - 1) / (size_t(c->world) * kThreads);
   int g = pick_blocks(c, rows, c->sm_count);
-  const long long min_world = c->params[B200_PARAM_NVLS_MIN_WORLD] >= 0 ? c->params[B200_PARAM_NVLS_MIN_WORLD] : 3;
-  const bool nvls = c->mc_active && c->world >= min_world;
+  const bool nvls = grad_nvls(c);
   if (!nvls) a.red_ctas = 0;  // peer-load reducers want the whole grid
   if (nvls) grad_allreduce_kernel<W, true><<<g, kThreads, 0, stream>>>(c->dev(), a);
   else grad_allreduce_kernel<W, false><<<g, kThreads, 0, stream>>>(c->dev(), a);
@@ -243,15 +243,10 @@ extern "C" int b200_grad_allreduce(b200_comm_t c, float *grad, size_t count, flo
   const size_t wire_es = b200_dtype_size(wire_dtype);
   // elements per launch so the wire image fits one staging slot (multiple of 8 elements)
   const size_t chunk_elems = (c->staging_bytes / wire_es) & ~size_t(7);
-  for (size_t done = 0; done < count;) {
-    const size_t n = (count - done) < chunk_elems ? (count - done) : chunk_elems;
-    const long long rc_param = c->params[B200_PARAM_NVLS_CTAS];
-    GradArgs a{grad + done, n, scale, c->staging_bytes, rc_param > 0 ? int(rc_param) : 0};
-    if (wire_dtype == B200_F32) rc = launch_grad<float>(c, a, stream);
-    else if (wire_dtype == B200_BF16) rc = launch_grad<__nv_bfloat16>(c, a, stream);
-    else rc = launch_grad<__half>(c, a, stream);
-    if (rc) return rc;
-    done += n;
-  }
-  return B200_OK;
+  return for_each_piece(count, chunk_elems, [&](size_t done, size_t n) {
+    GradArgs a{grad + done, n, scale, c->staging_bytes, nvls_ctas(c)};
+    if (wire_dtype == B200_F32) return launch_grad<float>(c, a, stream);
+    if (wire_dtype == B200_BF16) return launch_grad<__nv_bfloat16>(c, a, stream);
+    return launch_grad<__half>(c, a, stream);
+  });
 }

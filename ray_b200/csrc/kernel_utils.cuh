@@ -1,4 +1,5 @@
-// kernel_utils.cuh — copy/stage helpers and launch plumbing shared by the collective kernels.
+// kernel_utils.cuh — copy/stage helpers, argument checks and launch plumbing shared by the
+// collective kernels.  Launch decisions live in policy.h.
 #pragma once
 #include "comm.h"
 
@@ -58,13 +59,53 @@ __device__ __forceinline__ size_t staging_slot_offset(uint32_t launch, size_t st
   return (launch & 1u) ? staging_bytes : 0;
 }
 
-inline int pick_blocks(const b200_comm *c, size_t work_items, int cap) {
-  if (c->forced_blocks > 0) cap = c->forced_blocks;
-  size_t want = work_items < 1 ? 1 : work_items;
-  int g = int(want < size_t(cap) ? want : size_t(cap));
-  if (g > kMaxBlocks) g = kMaxBlocks;
-  return g < 1 ? 1 : g;
+// Argument checks of the entry points: each sets the error text and returns its status, or
+// B200_OK, so they chain as `if ((rc = check_a(..)) || (rc = check_b(..))) return rc;`.
+inline int check_dtype(int dtype, size_t *es) {
+  *es = b200_dtype_size(dtype);
+  if (*es == 0) {
+    set_error("unsupported dtype %d", dtype);
+    return B200_ERR_UNSUPPORTED;
+  }
+  return B200_OK;
 }
+
+inline int check_op(int op) {
+  if (op < 0 || op >= B200_OP_COUNT) {
+    set_error("unsupported reduce op %d", op);
+    return B200_ERR_UNSUPPORTED;
+  }
+  return B200_OK;
+}
+
+// `what`: "root", "peer" or "source"
+inline int check_rank(const b200_comm *c, int r, const char *what) {
+  if (r < 0 || r >= c->world) {
+    set_error("%s rank %d out of range for world size %d", what, r, c->world);
+    return B200_ERR_INVALID;
+  }
+  return B200_OK;
+}
+
+inline int null_tensor_error() {
+  set_error("null tensor pointer");
+  return B200_ERR_INVALID;
+}
+
+// Runs fn(done, n) -> status over [0, total) in pieces of at most `step` bytes (or elements),
+// in order; stops at the first failing piece.
+template <typename Fn>
+inline int for_each_piece(size_t total, size_t step, Fn fn) {
+  for (size_t done = 0; done < total;) {
+    const size_t n = (total - done) < step ? (total - done) : step;
+    if (int rc = fn(done, n)) return rc;
+    done += n;
+  }
+  return B200_OK;
+}
+
+// cudaFuncAttributeMaxDynamicSharedMemorySize = bulk-copy ring, once per (device, kernel)
+int set_dyn_smem(int device, const void *fn);
 
 #define B200_LAUNCH_CHECK(c)                                                     \
   do {                                                                           \

@@ -30,8 +30,7 @@
 #include <type_traits>
 
 #include "bulk_copy.cuh"
-#include "kernel_utils.cuh"
-#include "pipe.h"
+#include "policy.h"
 
 namespace b200 {
 
@@ -41,16 +40,6 @@ struct P2PArgs {
   size_t chunk;  // bytes per chunk of THIS message (<= slot size), same on both sides
   int peer;
 };
-
-// Chunk size is a pure function of the message size, so sender and receiver agree: big messages
-// use whole ring slots; mid-size ones are cut into kP2PRings pieces so that every CTA (one per
-// ring) carries one chunk and the message moves in parallel instead of through one CTA.
-inline size_t p2p_chunk_bytes(size_t nbytes, size_t slot_bytes) {
-  size_t c = (nbytes + kP2PRings - 1) / kP2PRings;
-  c = (c + 4095) & ~size_t(4095);
-  if (c < (size_t(16) << 10)) c = size_t(16) << 10;
-  return c < slot_bytes ? c : slot_bytes;
-}
 
 __device__ __forceinline__ bool cta_wait_flag(const DevComm &c, const uint32_t *flag, uint32_t target) {
   __shared__ int ok;
@@ -371,41 +360,26 @@ __global__ void __launch_bounds__(kThreads) get_ldst_kernel(GetArgs a) {
 }
 
 static int p2p_common(b200_comm *c, void *buf, size_t nbytes, int peer, cudaStream_t stream, bool send) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  if (peer < 0 || peer >= c->world) {
-    set_error("peer rank %d out of range for world size %d", peer, c->world);
-    return B200_ERR_INVALID;
-  }
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_rank(c, peer, "peer"))) return rc;
   if (peer == c->rank) {
     set_error("peer rank %d is this rank", peer);
     return B200_ERR_INVALID;
   }
   if (nbytes == 0) return B200_OK;
-  if (!buf) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!buf) return null_tensor_error();
   B200_CHECK_CUDA(cudaSetDevice(c->device));
-  const size_t chunk = p2p_chunk_bytes(nbytes, c->inbox_bytes / kP2PRings / kP2PSlots);
-  const size_t nchunks = (nbytes + chunk - 1) / chunk;
   // Grid is a pure function of the message size so both sides pair CTA b with CTA b.
-  int g = int(nchunks < size_t(kP2PRings) ? nchunks : size_t(kP2PRings));
-  P2PArgs a{static_cast<char *>(buf), nbytes, chunk, peer};
-  // The protocol (rings, slots, chunking) is a function of the message size alone; HOW this side
-  // moves its bytes is a local choice: the bulk-copy unit when the tensor is 16-byte aligned, a
-  // whole number of 16-byte units and the chunks are big enough to be worth a TMA pipeline.
-  const long long pb = c->params[B200_PARAM_P2P_BULK_MIN_CHUNK];
-  const size_t bulk_min_chunk = pb >= 0 ? size_t(pb) : (size_t(32) << 10);
-  const bool bulk = is_aligned16(buf) && (nbytes & 15) == 0 && chunk >= bulk_min_chunk && pb != 0;
-  if (bulk) {
+  const P2PPlan p = p2p_plan(c, buf, nbytes);
+  P2PArgs a{static_cast<char *>(buf), nbytes, p.chunk, peer};
+  if (p.bulk) {
     auto k = send ? p2p_bulk_kernel<true> : p2p_bulk_kernel<false>;
-    if (int rc2 = set_dyn_smem(c->device, reinterpret_cast<const void *>(k))) return rc2;
-    k<<<g, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a);
+    if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(k)))) return rc;
+    k<<<p.rings, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a);
   } else if (send) {
-    p2p_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
+    p2p_kernel<true><<<p.rings, kThreads, 0, stream>>>(c->dev(), a);
   } else {
-    p2p_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
+    p2p_kernel<false><<<p.rings, kThreads, 0, stream>>>(c->dev(), a);
   }
   B200_LAUNCH_CHECK(c);
   return B200_OK;
@@ -428,13 +402,9 @@ extern "C" int b200_recv(b200_comm_t c, void *buf, size_t nbytes, int peer, void
 
 extern "C" int b200_alltoall(b200_comm_t c, const void *const *ins, const size_t *send_counts, void *const *outs,
                              const size_t *recv_counts, int dtype, void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es))) return rc;
   if (!ins || !outs || !send_counts || !recv_counts) {
     set_error("null argument array");
     return B200_ERR_INVALID;
@@ -481,23 +451,15 @@ extern "C" int b200_alltoall(b200_comm_t c, const void *const *ins, const size_t
     B200_CHECK_CUDA(cudaMemcpyAsync(outs[0], ins[0], own_bytes, cudaMemcpyDeviceToDevice, stream));
     return B200_OK;
   }
-  // Ring count per role.  Both sides of a pair derive (chunk, G) from the message size, the world
-  // size and the grid cap alone, so b200_comm_set_blocks must be identical on every rank.  At most
-  // one CTA per SM keeps the grid co-resident even with the bulk roles' shared-memory ring.
-  int cap = c->forced_blocks > 0 ? c->forced_blocks : c->sm_count;
-  if (cap > c->sm_count) cap = c->sm_count;
   // Every role needs a CTA.  Checked against the world size rather than this call's counts, so all
   // ranks refuse together instead of one refusing while its peers wait for it.
+  const int cap = a2a_grid_cap(c);
   if (cap < 2 * (n - 1)) {
     set_error("all-to-all needs %d co-resident CTAs at world size %d but the grid is capped at %d "
               "(b200_comm_set_blocks)", 2 * (n - 1), n, cap);
     return B200_ERR_INVALID;
   }
-  int kcap = cap / (2 * (n - 1));
-  kcap = kcap < 1 ? 1 : (kcap > kP2PRings ? kP2PRings : kcap);
-  const size_t slot_bytes = c->inbox_bytes / kP2PRings / kP2PSlots;
-  const long long pb = c->params[B200_PARAM_P2P_BULK_MIN_CHUNK];
-  const size_t bulk_min_chunk = pb >= 0 ? size_t(pb) : (size_t(32) << 10);
+  const int kcap = a2a_ring_cap(c, cap);
   A2AArgs a{};
   int grid = 0;
   bool any_bulk = false;
@@ -507,20 +469,12 @@ extern "C" int b200_alltoall(b200_comm_t c, const void *const *ins, const size_t
       const size_t nbytes = (send ? send_counts[peer] : recv_counts[peer]) * es;
       if (nbytes == 0) continue;
       char *buf = send ? const_cast<char *>(static_cast<const char *>(ins[peer])) : static_cast<char *>(outs[peer]);
-      const size_t chunk = p2p_chunk_bytes(nbytes, slot_bytes);
-      const size_t nchunks = (nbytes + chunk - 1) / chunk;
-      A2ARole &r = a.role[a.nroles++];
-      r.buf = buf;
-      r.nbytes = nbytes;
-      r.chunk = chunk;
-      r.peer = peer;
-      r.first = grid;
-      r.G = int(nchunks < size_t(kcap) ? nchunks : size_t(kcap));
-      r.send = send;
-      // the mechanism p2p_common would choose for this transfer alone
-      r.bulk = is_aligned16(buf) && (nbytes & 15) == 0 && chunk >= bulk_min_chunk && pb != 0;
-      any_bulk = any_bulk || r.bulk;
-      grid += r.G;
+      // what b200_send / b200_recv would do with this transfer alone, on at most kcap rings
+      const P2PPlan p = p2p_plan(c, buf, nbytes);
+      const int G = p.rings < kcap ? p.rings : kcap;
+      a.role[a.nroles++] = A2ARole{buf, nbytes, p.chunk, peer, grid, G, send, p.bulk};
+      any_bulk = any_bulk || p.bulk;
+      grid += G;
     }
   }
   // grid <= 2(n-1) * kcap <= cap here
@@ -528,15 +482,14 @@ extern "C" int b200_alltoall(b200_comm_t c, const void *const *ins, const size_t
   a.own_src = static_cast<const char *>(ins[me]);
   a.own_dst = static_cast<char *>(outs[me]);
   a.own_bytes = own_bytes;
-  // Every CTA copies a slice of the own segment.  A large own segment gets extra copy-only CTAs, up
-  // to one per 64 KiB and within the cap: a local copy of MiBs next to small remote messages would
-  // otherwise crawl through the few role CTAs.  Copy-only CTAs never wait.
-  const size_t own_ctas = (own_bytes + (size_t(64) << 10) - 1) / (size_t(64) << 10);
+  // Every CTA copies a slice of the own segment; a large one gets extra copy-only CTAs, within the
+  // cap.  Copy-only CTAs never wait.
+  const size_t own_ctas = a2a_own_ctas(own_bytes);
   if (own_ctas > size_t(grid)) grid = int(own_ctas < size_t(cap) ? own_ctas : size_t(cap));
   a.own_bulk = grid > a.role_ctas && is_aligned16(a.own_src) && is_aligned16(a.own_dst) && (own_bytes & 15) == 0;
   any_bulk = any_bulk || a.own_bulk;
   if (any_bulk) {
-    if (int rc2 = set_dyn_smem(c->device, reinterpret_cast<const void *>(alltoall_kernel))) return rc2;
+    if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(alltoall_kernel)))) return rc;
     alltoall_kernel<<<grid, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a);
   } else {
     alltoall_kernel<<<grid, kThreads, 0, stream>>>(c->dev(), a);
@@ -554,30 +507,23 @@ extern "C" int b200_symm_base(b200_comm_t c, void **base, size_t *bytes) {
 }
 
 extern "C" int b200_get(b200_comm_t c, void *dst, int src_rank, size_t src_heap_offset, size_t nbytes, void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  if (src_rank < 0 || src_rank >= c->world) {
-    set_error("source rank %d out of range for world size %d", src_rank, c->world);
-    return B200_ERR_INVALID;
-  }
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_rank(c, src_rank, "source"))) return rc;
   if (src_heap_offset + nbytes > c->heap_bytes) {
     set_error("[%zu, %zu) is outside the %zu-byte symmetric heap", src_heap_offset, src_heap_offset + nbytes,
               c->heap_bytes);
     return B200_ERR_INVALID;
   }
   if (nbytes == 0) return B200_OK;
-  if (!dst) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!dst) return null_tensor_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   GetArgs a{reinterpret_cast<const char *>(c->data.va[src_rank]) + 2 * c->staging_bytes + src_heap_offset,
-            static_cast<char *>(dst), nbytes, size_t(256) << 10};
-  if (is_aligned16(a.src) && is_aligned16(a.dst) && (nbytes & 15) == 0 && nbytes >= (size_t(256) << 10)) {
+            static_cast<char *>(dst), nbytes, kGetSegBytes};
+  if (get_bulk(a.src, a.dst, nbytes)) {
     const size_t nseg = (nbytes + a.seg_bytes - 1) / a.seg_bytes;
     const int g = int(nseg < 16 ? nseg : 16);
-    if (int rc2 = set_dyn_smem(c->device, reinterpret_cast<const void *>(get_bulk_kernel))) return rc2;
+    if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(get_bulk_kernel)))) return rc;
     get_bulk_kernel<<<g, kThreads, kBulkSmemBytes, stream>>>(a);
   } else {
     const size_t U = make_units(nbytes).total();

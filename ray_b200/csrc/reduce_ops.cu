@@ -6,7 +6,7 @@
 // NVLink (the local copy-in and the transfer are the same instruction stream).  After
 // one barrier every rank reduces its n sub-slots from local HBM, rank-ascending, into
 // the caller's output tensor.
-#include "kernel_utils.cuh"
+#include "policy.h"
 
 namespace b200 {
 
@@ -146,22 +146,11 @@ using namespace b200;
 
 extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *out, size_t count,
                                   int dtype, int op, void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
-  if (op < 0 || op >= B200_OP_COUNT) {
-    set_error("unsupported reduce op %d", op);
-    return B200_ERR_UNSUPPORTED;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op))) return rc;
   if (count == 0) return B200_OK;
-  if (!ins || !out) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!ins || !out) return null_tensor_error();
   for (int p = 0; p < c->world; ++p)
     if (!ins[p]) {
       set_error("input tensor %d is null", p);
@@ -174,54 +163,36 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
     if (ins[0] != out) B200_CHECK_CUDA(cudaMemcpyAsync(out, ins[0], total, cudaMemcpyDeviceToDevice, stream));
     return B200_OK;
   }
-  // n sub-slots of the chunk must fit one staging slot; keep chunks 16-byte multiples
-  size_t chunk_max = (c->staging_bytes / size_t(c->world)) & ~size_t(15);
-  for (size_t done = 0; done < total;) {
-    const size_t nbytes = (total - done) < chunk_max ? (total - done) : chunk_max;
+  // n sub-slots of the piece must fit one staging slot; keep pieces 16-byte multiples
+  const size_t step = (c->staging_bytes / size_t(c->world)) & ~size_t(15);
+  return for_each_piece(total, step, [&](size_t done, size_t nbytes) -> int {
     RSArgs a{};
     for (int p = 0; p < c->world; ++p) a.ins[p] = static_cast<const char *>(ins[p]) + done;
     a.out = static_cast<char *>(out) + done;
     a.nbytes = nbytes;
     a.staging_bytes = c->staging_bytes;
-    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc = launch_rs<T, OP>(c, a, stream); }));
-    if (rc) return rc;
-    done += nbytes;
-  }
-  return B200_OK;
+    int rc2 = B200_OK;
+    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc2 = launch_rs<T, OP>(c, a, stream); }));
+    return rc2;
+  });
 }
 
 extern "C" int b200_reduce(b200_comm_t c, void *buf, size_t count, int dtype, int op, int root,
                            void *stream_) {
-  int rc = check_usable(c);
-  if (rc) return rc;
-  const size_t es = b200_dtype_size(dtype);
-  if (es == 0) {
-    set_error("unsupported dtype %d", dtype);
-    return B200_ERR_UNSUPPORTED;
-  }
-  if (op < 0 || op >= B200_OP_COUNT) {
-    set_error("unsupported reduce op %d", op);
-    return B200_ERR_UNSUPPORTED;
-  }
-  if (root < 0 || root >= c->world) {
-    set_error("root rank %d out of range for world size %d", root, c->world);
-    return B200_ERR_INVALID;
-  }
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op)) ||
+      (rc = check_rank(c, root, "root")))
+    return rc;
   if (count == 0) return B200_OK;
-  if (!buf) {
-    set_error("null tensor pointer");
-    return B200_ERR_INVALID;
-  }
+  if (!buf) return null_tensor_error();
   if (c->world == 1) return B200_OK;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
-  const size_t total = count * es;
-  for (size_t done = 0; done < total;) {
-    const size_t nbytes = (total - done) < c->staging_bytes ? (total - done) : c->staging_bytes;
+  return for_each_piece(count * es, c->staging_bytes, [&](size_t done, size_t nbytes) -> int {
     ReduceArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
-    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc = launch_reduce<T, OP>(c, a, stream); }));
-    if (rc) return rc;
-    done += nbytes;
-  }
-  return B200_OK;
+    int rc2 = B200_OK;
+    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc2 = launch_reduce<T, OP>(c, a, stream); }));
+    return rc2;
+  });
 }
