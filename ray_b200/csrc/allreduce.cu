@@ -38,7 +38,6 @@ struct ARArgs {
 // ---------------------------------------------------------------------------
 template <typename T, int OP>
 __global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm c, ARArgs a) {
-  using Tr = Traits<T>;
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const int n = c.world, r = c.rank;
@@ -62,12 +61,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm 
 #pragma unroll
     for (int p = 0; p < kMaxRanks; ++p)
       if (p < n) v[p] = ld_peer(c.data[p] + off + (u << 4));
-    typename Tr::Acc acc = Tr::unpack(v[0]);
-#pragma unroll
-    for (int p = 1; p < kMaxRanks; ++p)
-      if (p < n) Tr::template reduce<OP>(acc, Tr::unpack(v[p]));
-    if (OP == B200_AVG) Tr::average(acc, n);
-    store_user_unit(a.out, u, un, out_al, Tr::pack(acc));
+    store_user_unit(a.out, u, un, out_al, reduce_ranks<T, OP>(v, n));
   }
   finish_launch(c);
 }

@@ -1,5 +1,7 @@
 // allreduce_core.cuh — the reduce-and-publish phase shared by the two-shot / NVLS all-reduce,
-// the fused gradient kernel and the multi-tensor kernel.
+// the fused gradient kernel and the multi-tensor kernel.  Its per-unit steps, nvls_finish and
+// publish_unit, also serve the reduce workers of the pipelined all-reduce (allreduce_pipe.cu); the
+// rank-ascending reduce itself is reduce_ranks (common.cuh).
 //
 // Work decomposition (see DESIGN.md §4): the staged message is U 16-byte units, cut into rows
 // of n*kThreads units.  CTA b handles rows b, b+G, ...; inside a row rank r owns the kThreads
@@ -22,12 +24,35 @@ __device__ __forceinline__ RowGeom make_rows(size_t U, int n) {
   return g;
 }
 
+// multimem.ld_reduce returns the sum over the n ranks; AVG divides it here, before multimem.st.
+template <typename T, int OP>
+__device__ __forceinline__ uint4 nvls_finish(uint4 v, int n) {
+  if (OP != B200_AVG) return v;
+  using Tr = Traits<T>;
+  typename Tr::Acc acc = Tr::unpack(v);
+  Tr::average(acc, n);
+  return Tr::pack(acc);
+}
+
+// Store `v` as unit u at byte offset `off` of every rank's data region: the local copy first, then
+// the peers in ring order.  n and r are the caller's copies of c.world and c.rank, read before its
+// loads: reading them here, after the loads' memory clobbers, compiles the AVG kernels differently.
+__device__ __forceinline__ void publish_unit(const DevComm &c, int n, int r, size_t off, size_t u, uint4 v) {
+#pragma unroll
+  for (int i = 0; i < kMaxRanks; ++i) {
+    if (i < n) {
+      int p = r + i;
+      if (p >= n) p -= n;
+      st_vec(c.data[p] + off + (u << 4), v);
+    }
+  }
+}
+
 // Reduce the units this rank owns across all n ranks' buffers at offset `off` of the data
 // region and publish the result into every rank's buffer at the same offset.
 template <typename T, int OP, bool NVLS>
 __device__ __forceinline__ void reduce_publish_rows(const DevComm &c, size_t off, const RowGeom &g,
                                                     size_t G = 0) {
-  using Tr = Traits<T>;
   const int n = c.world, r = c.rank, t = threadIdx.x;
   if (G == 0) G = gridDim.x;  // CTAs [0, G) share the rows of this phase
   if (NVLS) {
@@ -46,11 +71,7 @@ __device__ __forceinline__ void reduce_publish_rows(const DevComm &c, size_t off
         const size_t row = row0 + size_t(j) * G;
         const size_t u = row * g.row_units + size_t(r) * kThreads + t;
         if (row < g.R && u < g.U) {
-          if (OP == B200_AVG) {
-            typename Tr::Acc acc = Tr::unpack(v[j]);
-            Tr::average(acc, n);
-            v[j] = Tr::pack(acc);
-          }
+          v[j] = nvls_finish<T, OP>(v[j], n);
           multimem_st(mc + (u << 4), v[j]);
         }
       }
@@ -73,22 +94,7 @@ __device__ __forceinline__ void reduce_publish_rows(const DevComm &c, size_t off
       for (int j = 0; j < UNR; ++j) {
         const size_t row = row0 + size_t(j) * G;
         const size_t u = row * g.row_units + size_t(r) * kThreads + t;
-        if (row < g.R && u < g.U) {
-          typename Tr::Acc acc = Tr::unpack(v[j][0]);
-#pragma unroll
-          for (int p = 1; p < kMaxRanks; ++p)
-            if (p < n) Tr::template reduce<OP>(acc, Tr::unpack(v[j][p]));  // rank-ascending
-          if (OP == B200_AVG) Tr::average(acc, n);
-          const uint4 res = Tr::pack(acc);
-#pragma unroll
-          for (int i = 0; i < kMaxRanks; ++i) {
-            if (i < n) {
-              int p = r + i;  // local copy first, then walk the peers
-              if (p >= n) p -= n;
-              st_vec(c.data[p] + off + (u << 4), res);
-            }
-          }
-        }
+        if (row < g.R && u < g.U) publish_unit(c, n, r, off, u, reduce_ranks<T, OP>(v[j], n));
       }
     }
   }

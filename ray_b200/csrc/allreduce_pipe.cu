@@ -279,7 +279,6 @@ struct ItemIter {
 template <typename T, int OP, bool NVLS>
 __global__ void __launch_bounds__(kThreads + 32, 1) allreduce_pipe_kernel(DevComm c, PipeArgs a) {
   extern __shared__ __align__(128) char dyn_smem[];
-  using Tr = Traits<T>;
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const size_t off = staging_slot_offset(launch, a.staging_bytes);
@@ -357,11 +356,7 @@ __global__ void __launch_bounds__(kThreads + 32, 1) allreduce_pipe_kernel(DevCom
           for (int q = 0; q < kItemUnroll; ++q) {
             const size_t u = u0 + size_t(q) * kThreads;
             if (u < hi) {
-              if (OP == B200_AVG) {
-                typename Tr::Acc acc = Tr::unpack(v[q]);
-                Tr::average(acc, n);
-                v[q] = Tr::pack(acc);
-              }
+              v[q] = nvls_finish<T, OP>(v[q], n);
               multimem_st(mc + (u << 4), v[q]);
             }
           }
@@ -381,22 +376,7 @@ __global__ void __launch_bounds__(kThreads + 32, 1) allreduce_pipe_kernel(DevCom
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
               const size_t u = u0 + size_t(q0 + q) * kThreads;
-              if (u < hi) {
-                typename Tr::Acc acc = Tr::unpack(v[q][0]);
-#pragma unroll
-                for (int p = 1; p < kMaxRanks; ++p)
-                  if (p < n) Tr::template reduce<OP>(acc, Tr::unpack(v[q][p]));  // rank-ascending
-                if (OP == B200_AVG) Tr::average(acc, n);
-                const uint4 res = Tr::pack(acc);
-#pragma unroll
-                for (int i = 0; i < kMaxRanks; ++i) {
-                  if (i < n) {
-                    int p = r + i;
-                    if (p >= n) p -= n;
-                    st_vec(c.data[p] + cbase + (u << 4), res);
-                  }
-                }
-              }
+              if (u < hi) publish_unit(c, n, r, cbase, u, reduce_ranks<T, OP>(v[q], n));
             }
           }
         }

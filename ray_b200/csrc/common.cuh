@@ -360,6 +360,19 @@ template <> __device__ __forceinline__ __nv_bfloat16 HalfTraits<__nv_bfloat16>::
 template <> struct Traits<__half> : HalfTraits<__half> {};
 template <> struct Traits<__nv_bfloat16> : HalfTraits<__nv_bfloat16> {};
 
+// v[0] (op) v[1] (op) ... (op) v[n-1], then AVG's division, packed.  The fixed rank-ascending order
+// is what makes floating-point SUM / PROD bit-exact against the reference (DESIGN.md §2).
+template <typename T, int OP>
+__device__ __forceinline__ uint4 reduce_ranks(const uint4 (&v)[kMaxRanks], int n) {
+  using Tr = Traits<T>;
+  typename Tr::Acc acc = Tr::unpack(v[0]);
+#pragma unroll
+  for (int p = 1; p < kMaxRanks; ++p)
+    if (p < n) Tr::template reduce<OP>(acc, Tr::unpack(v[p]));
+  if (OP == B200_AVG) Tr::average(acc, n);
+  return Tr::pack(acc);
+}
+
 // ---------------------------------------------------------------------------
 // NVLS reduction: one instruction pulls the same 16 bytes from every rank's
 // buffer, reduced inside the switch.  Available for SUM on f32 / f16 / bf16

@@ -19,7 +19,6 @@ struct RSArgs {
 
 template <typename T, int OP>
 __global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, RSArgs a) {
-  using Tr = Traits<T>;
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const int n = c.world, r = c.rank;
@@ -63,12 +62,7 @@ __global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, R
 #pragma unroll
     for (int p = 0; p < kMaxRanks; ++p)
       if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
-    typename Tr::Acc acc = Tr::unpack(v[0]);
-#pragma unroll
-    for (int p = 1; p < kMaxRanks; ++p)
-      if (p < n) Tr::template reduce<OP>(acc, Tr::unpack(v[p]));
-    if (OP == B200_AVG) Tr::average(acc, n);
-    store_user_unit(a.out, u, un, out_al, Tr::pack(acc));
+    store_user_unit(a.out, u, un, out_al, reduce_ranks<T, OP>(v, n));
   }
   finish_launch(c);
 }
@@ -83,7 +77,6 @@ struct ReduceArgs {
 // Every rank stages its tensor; the root pulls all n copies and reduces in place.
 template <typename T, int OP>
 __global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceArgs a) {
-  using Tr = Traits<T>;
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const int n = c.world, r = c.rank;
@@ -108,12 +101,7 @@ __global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceAr
 #pragma unroll
       for (int p = 0; p < kMaxRanks; ++p)
         if (p < n) v[p] = ld_peer(c.data[p] + off + (u << 4));
-      typename Tr::Acc acc = Tr::unpack(v[0]);
-#pragma unroll
-      for (int p = 1; p < kMaxRanks; ++p)
-        if (p < n) Tr::template reduce<OP>(acc, Tr::unpack(v[p]));
-      if (OP == B200_AVG) Tr::average(acc, n);
-      store_user_unit(a.buf, u, un, al, Tr::pack(acc));
+      store_user_unit(a.buf, u, un, al, reduce_ranks<T, OP>(v, n));
     }
   }
   finish_launch(c);
