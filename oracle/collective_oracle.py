@@ -85,17 +85,25 @@ def reduce_rank_ascending(tensors: Sequence[np.ndarray], op: int, accumulate: st
                 result = (result + t).astype(work, copy=False)
             elif op == PRODUCT:
                 result = (result * t).astype(work, copy=False)
-            elif op == MAX:
-                result = np.maximum(result, t)
-            elif op == MIN:
-                result = np.minimum(result, t)
+            elif op in (MIN, MAX):
+                # Spelled out rather than np.minimum / np.maximum, whose pick between equal operands
+                # (+0.0 / -0.0) differs by dtype (numpy 2.3: the second for fp32/fp64/bf16, the
+                # first for fp16).  Rule: a NaN from any rank propagates; on a tie the lower ranks'
+                # value is kept.
+                better = (t < result) if op == MIN else (t > result)
+                if not np.issubdtype(np.dtype(work), np.integer):
+                    better |= np.isnan(t) & ~np.isnan(result)
+                result = np.where(better, t, result)
             else:
                 raise ValueError(f"Operation {op} not supported")
         if op == AVG:
             n = len(tensors)
             if np.issubdtype(np.dtype(work), np.integer):
-                # truncating division, as an integer ncclAvg does
-                result = (np.trunc(result.astype(np.float64) / n)).astype(work)
+                # the wrapped sum divided with truncation toward zero, as an integer ncclAvg does;
+                # in integer arithmetic, since a float64 detour loses int64/uint64 sums above 2**53
+                div = np.asarray(n, dtype=work)
+                q = result // div  # floor division; one more toward zero for a negative inexact quotient
+                result = (q + ((result % div != 0) & (result < 0)).astype(work)).astype(work, copy=False)
             else:
                 result = (result / np.asarray(n, dtype=work)).astype(work, copy=False)
         return result.astype(dtype, copy=False)
@@ -185,10 +193,11 @@ def cgraph_reducescatter(per_rank: List[np.ndarray], cgraph_op: int, accumulate:
 # Data-parallel gradient synchronisation (the path TorchTrainer / LearnerGroup ride)
 # ---------------------------------------------------------------------------
 def _round_to(x: np.ndarray, dtype: np.dtype) -> np.ndarray:
-    return x.astype(dtype).astype(np.float32)
+    with np.errstate(over="ignore"):  # beyond the type's range rounds to inf, as the kernels do
+        return x.astype(dtype).astype(np.float32)
 
 
-def ddp_grad_sync(per_rank_grads: List[np.ndarray], wire: str = "f32") -> List[np.ndarray]:
+def ddp_grad_sync(per_rank_grads: List[np.ndarray], wire: str = "f32", scale=None) -> List[np.ndarray]:
     """Mean of fp32 gradient buckets as torch DDP computes it under ray.train
     (train/torch/train_loop_utils.py:456-480 wraps the model in DDP; the c10d reducer
     divides each bucket by world_size and all-reduces it with SUM).
@@ -198,9 +207,12 @@ def ddp_grad_sync(per_rank_grads: List[np.ndarray], wire: str = "f32") -> List[n
     divide by n in the wire type, sum, cast back to fp32.  The kernel multiplies by 1/n in
     fp32 *before* the cast; for power-of-two n both orders are bit-identical (barring
     subnormals) and the kernel accumulates the sum in fp32.
+
+    ``scale`` replaces 1/n by another fp32 factor (the kernel's ``scale`` argument): every
+    gradient is multiplied by it in fp32, then cast to the wire type, as above.
     """
     n = len(per_rank_grads)
-    inv = np.float32(1.0) / np.float32(n)
+    inv = np.float32(1.0) / np.float32(n) if scale is None else np.float32(scale)
     if wire == "f32":
         scaled = [(g.astype(np.float32) * inv).astype(np.float32) for g in per_rank_grads]
         red = reduce_rank_ascending(scaled, SUM)

@@ -272,8 +272,11 @@ template <int OP, typename A>
 __device__ __forceinline__ A combine(A a, A b) {
   if (OP == B200_SUM || OP == B200_AVG) return a + b;
   if (OP == B200_PROD) return a * b;
-  if (OP == B200_MIN) return b < a ? b : a;
-  return b > a ? b : a;  // MAX
+  // MIN / MAX propagate a NaN from any rank, as np.minimum / np.maximum do: a NaN accumulator
+  // survives because every comparison with it is false, and `b != b` picks up a NaN operand (it
+  // is always false for the integer types, so their instructions do not change).
+  if (OP == B200_MIN) return (b < a || b != b) ? b : a;
+  return (b > a || b != b) ? b : a;  // MAX
 }
 
 template <typename T>
