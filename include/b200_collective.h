@@ -220,6 +220,16 @@ int b200_get(b200_comm_t comm, void *dst, int src_rank, size_t src_heap_offset, 
 int b200_grad_allreduce(b200_comm_t comm, float *grad, size_t count, float scale,
                         int wire_dtype, void *stream);
 
+/* Fused sharded gradient synchronisation (FSDP / ZeRO counterpart of b200_grad_allreduce):
+ * grad holds world_size * count fp32 elements (rank q's stripe at grad + q * count); out (count
+ * elements) receives sum_r wire(grad_r[this rank's stripe] * scale), cast back to fp32 -- bit for
+ * bit this rank's stripe of what b200_grad_allreduce leaves in the bucket on the peer path.  One
+ * launch per piece of at most staging_bytes / world_size bytes of wire data per rank.  out may be
+ * this rank's own stripe (grad + rank * count) but must not overlap grad otherwise.  Replaces
+ * FSDP's div + fp32 ncclReduceScatter + div (and its compress-hook casts). */
+int b200_grad_reducescatter(b200_comm_t comm, const float *grad, float *out, size_t count,
+                            float scale, int wire_dtype, void *stream);
+
 /* Multi-tensor all-reduce (SURVEY K9): reduces `ntensors` same-dtype tensors as one
  * message without a host-side flatten (replaces parameters_to_vector + views at
  * dag/collective_node.py:220-232).  ptrs/counts are host arrays. */

@@ -94,6 +94,7 @@ SIGNATURES = {
     "b200_symm_base": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t)]),
     "b200_get": (c_int, [c_void_p, c_void_p, c_int, c_size_t, c_size_t, c_void_p]),
     "b200_grad_allreduce": (c_int, [c_void_p, c_void_p, c_size_t, c_float, c_int, c_void_p]),
+    "b200_grad_reducescatter": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_float, c_int, c_void_p]),
     "b200_allreduce_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, c_int, c_int, c_void_p]),
     "b200_last_error": (c_char_p, []),
     "b200_version": (c_char_p, []),

@@ -385,6 +385,20 @@ class B200Comm:
         N.check(self._lib.b200_grad_allreduce(self._h, grad.data_ptr(), grad.numel(), float(scale),
                                               dtype_code(wire_dtype), self._stream()))
 
+    def grad_reducescatter(self, out: torch.Tensor, grad: torch.Tensor, scale: float,
+                           wire_dtype: torch.dtype = torch.bfloat16) -> None:
+        """Fused sharded gradient sync (the FSDP / ZeRO counterpart of ``grad_allreduce``):
+        ``out = sum_r wire(grad_r[this rank's 1/world slice] * scale)``, cast back to fp32.
+        ``out`` may be this rank's own slice of ``grad`` (in place), but no other part of it."""
+        _check_cuda_contiguous(grad)
+        _check_cuda_contiguous(out, "output tensor")
+        if grad.dtype != torch.float32 or out.dtype != torch.float32:
+            raise RuntimeError("grad_reducescatter expects float32 gradient and output tensors")
+        if grad.numel() != out.numel() * self.world_size:
+            raise RuntimeError("grad_reducescatter input must hold world_size slices of the output size")
+        N.check(self._lib.b200_grad_reducescatter(self._h, grad.data_ptr(), out.data_ptr(), out.numel(),
+                                                  float(scale), dtype_code(wire_dtype), self._stream()))
+
     def allreduce_multi(self, tensors: List[torch.Tensor], op: int = N.SUM) -> None:
         if not tensors:
             return

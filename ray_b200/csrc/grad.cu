@@ -218,6 +218,113 @@ static int launch_grad(b200_comm *c, GradArgs a, cudaStream_t stream) {
   return B200_OK;
 }
 
+// ---------------------------------------------------------------------------
+// Fused sharded gradient synchronisation (FSDP / ZeRO): the reduce-scatter counterpart of
+// grad_allreduce_kernel, with the push design of reducescatter_kernel (reduce_ops.cu).  Rank r
+// scales and casts stripe q of its gradient and stores it into sub-slot r of rank q's staging slot
+// (wire bytes: half of an fp32 reduce-scatter's for bf16 / f16); after one barrier every rank
+// reduces its n sub-slots rank-ascending in fp32, rounds once to the wire type and writes fp32.
+// That is grad_allreduce_kernel's peer-path arithmetic restricted to this rank's stripe, so the
+// shard is bit-identical to the same elements of the all-reduced bucket.
+// ---------------------------------------------------------------------------
+struct GradRSArgs {
+  const float *grad;  // element 0 of this piece in stripe 0; stripe q starts `stride` elements later per q
+  float *out;
+  size_t stride;  // elements per stripe (the shard size)
+  size_t count;   // elements of this piece
+  float scale;
+  size_t staging_bytes;
+};
+
+template <typename W>
+__global__ void __launch_bounds__(kThreads, 1) grad_reducescatter_kernel(DevComm c, GradRSArgs a) {
+  constexpr int E = Wire<W>::kElems;
+  const uint32_t launch = c.st->launch_ctr;
+  const uint32_t ep = launch * 4u;
+  const int n = c.world, r = c.rank;
+  const size_t U = (a.count + E - 1) / E;
+  const size_t sub = U << 4;  // bytes per sub-slot
+  const size_t off = staging_slot_offset(launch, a.staging_bytes);
+  const size_t step = size_t(gridDim.x) * kThreads;
+  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
+
+  // push: stripe (r+i)%n goes to rank (r+i)%n, sub-slot r.  Stripes of a shard size that is not a
+  // multiple of 4 are not all 16-byte aligned, so alignment is taken per stripe.
+  for (size_t u = first; u < U; u += step) {
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int q = r + i;
+        if (q >= n) q -= n;
+        const float *s = a.grad + size_t(q) * a.stride;
+        v[i] = load_grad_unit<W>(s, u, a.count, a.scale, is_aligned16(s));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int q = r + i;
+        if (q >= n) q -= n;
+        st_vec(c.data[q] + off + size_t(r) * sub + (u << 4), v[i]);
+      }
+    }
+  }
+
+  if (!cta_barrier_all(c, ep + 1)) {
+    finish_launch(c);
+    return;
+  }
+
+  // Every thread writes exactly the units it read from its own stripe before the barrier, so `out`
+  // may be that stripe.
+  const bool out_al = is_aligned16(a.out);
+  const char *mine = c.data[r] + off;
+  for (size_t u = first; u < U; u += step) {
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int p = 0; p < kMaxRanks; ++p)
+      if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
+    store_grad_unit<W>(a.out, u, a.count, out_al, reduce_ranks<W, B200_SUM>(v, n));
+  }
+  finish_launch(c);
+}
+
+template <typename W>
+__device__ __forceinline__ float wire_round(float f) {
+  if constexpr (std::is_same<W, __nv_bfloat16>::value) return __bfloat162float(__float2bfloat16_rn(f));
+  else if constexpr (std::is_same<W, __half>::value) return __half2float(__float2half_rn(f));
+  else return f;
+}
+
+// world == 1: out = wire(grad * scale), out of place or in place, any alignment.  One thread per
+// 4 elements; 16-byte accesses where both pointers allow them.
+template <typename W>
+__global__ void __launch_bounds__(kLocalThreads) grad_rs_local_kernel(GradRSArgs a) {
+  const size_t e0 = (size_t(blockIdx.x) * kLocalThreads + threadIdx.x) * 4;
+  if (e0 >= a.count) return;
+  if (is_aligned16(a.grad) && is_aligned16(a.out) && e0 + 4 <= a.count) {
+    st_vec(a.out + e0, wire_round_trip<W>(ld_stream(a.grad + e0), a.scale));
+    return;
+  }
+  for (size_t i = e0; i < e0 + 4 && i < a.count; ++i) a.out[i] = wire_round<W>(a.grad[i] * a.scale);
+}
+
+template <typename W>
+static int launch_grad_rs(b200_comm *c, const GradRSArgs &a, cudaStream_t stream) {
+  if (c->world == 1) {
+    const size_t threads = (a.count + 3) / 4;
+    grad_rs_local_kernel<W><<<unsigned((threads + kLocalThreads - 1) / kLocalThreads), kLocalThreads, 0, stream>>>(a);
+  } else {
+    constexpr int E = Wire<W>::kElems;
+    const size_t U = (a.count + E - 1) / E;
+    const int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
+    grad_reducescatter_kernel<W><<<g, kThreads, 0, stream>>>(c->dev(), a);
+  }
+  B200_LAUNCH_CHECK(c);
+  return B200_OK;
+}
+
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
 const void *grad_module_anchor() { return reinterpret_cast<const void *>(&grad_local_scalar_kernel<float>); }
 
@@ -248,5 +355,39 @@ extern "C" int b200_grad_allreduce(b200_comm_t c, float *grad, size_t count, flo
     if (wire_dtype == B200_F32) return launch_grad<float>(c, a, stream);
     if (wire_dtype == B200_BF16) return launch_grad<__nv_bfloat16>(c, a, stream);
     return launch_grad<__half>(c, a, stream);
+  });
+}
+
+extern "C" int b200_grad_reducescatter(b200_comm_t c, const float *grad, float *out, size_t count, float scale,
+                                       int wire_dtype, void *stream_) {
+  int rc = check_usable(c);
+  if (rc) return rc;
+  if (wire_dtype != B200_F32 && wire_dtype != B200_BF16 && wire_dtype != B200_F16) {
+    set_error("wire dtype must be f32, bf16 or f16 (got %d)", wire_dtype);
+    return B200_ERR_UNSUPPORTED;
+  }
+  if (count == 0) return B200_OK;
+  if (!grad) {
+    set_error("null gradient pointer");
+    return B200_ERR_INVALID;
+  }
+  if (!out) {
+    set_error("null output pointer");
+    return B200_ERR_INVALID;
+  }
+  // the one overlap that is safe: out IS this rank's stripe (each unit is read before it is written)
+  const float *own = grad + size_t(c->rank) * count;
+  if (out != own && out < grad + size_t(c->world) * count && grad < out + count) {
+    set_error("output overlaps the gradient other than as this rank's stripe (rank %d)", c->rank);
+    return B200_ERR_INVALID;
+  }
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  const size_t piece = c->world == 1 ? count : grad_rs_piece_elems(c, b200_dtype_size(wire_dtype));
+  return for_each_piece(count, piece, [&](size_t done, size_t m) {
+    GradRSArgs a{grad + done, out + done, count, m, scale, c->staging_bytes};
+    if (wire_dtype == B200_F32) return launch_grad_rs<float>(c, a, stream);
+    if (wire_dtype == B200_BF16) return launch_grad_rs<__nv_bfloat16>(c, a, stream);
+    return launch_grad_rs<__half>(c, a, stream);
   });
 }

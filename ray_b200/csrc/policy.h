@@ -162,6 +162,15 @@ inline bool grad_nvls(const b200_comm *c) {
   return c->mc_active && c->world >= (v >= 0 ? v : 3);
 }
 
+// Shard elements per launch of the fused gradient reduce-scatter: the n sub-slots of a piece,
+// ceil(m / E) 16-byte wire units each (E = 16 / wire element size), fill at most one staging slot.
+// A multiple of 8 elements, so every piece starts on a whole wire unit and keeps its stripe's
+// 16-byte alignment.
+inline size_t grad_rs_piece_elems(const b200_comm *c, size_t wire_es) {
+  const size_t units = c->staging_bytes / (size_t(c->world) * 16);
+  return (units * (16 / wire_es)) & ~size_t(7);
+}
+
 // ---- point-to-point, all-to-all, get (p2p.cu) ------------------------------------------------
 
 // Chunk size is a pure function of the message size, so sender and receiver agree: big messages

@@ -423,6 +423,13 @@ class B200ProcessGroup(dist.ProcessGroup):
         work = self._run([bucket], lambda comm: comm.grad_allreduce(bucket, scale, wire_dtype), bucket, tag="grad")
         return work.get_future()
 
+    def grad_reducescatter(self, out: torch.Tensor, grad: torch.Tensor, scale: float,
+                           wire_dtype: torch.dtype) -> B200Work:
+        """Fused scale + wire cast + reduce-scatter + cast back: ``out`` receives this rank's shard
+        of the scaled sum of the flat fp32 ``grad`` (world_size * out.numel() elements)."""
+        return self._run([out, grad], lambda comm: comm.grad_reducescatter(out, grad, scale, wire_dtype), out,
+                         tag="grad")
+
     # ------------------------------------------------------------------ lifecycle
     def abort(self):
         if self._comm is not None:

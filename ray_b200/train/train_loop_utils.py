@@ -6,7 +6,9 @@ move the module to this worker's device, then wrap it in ``DistributedDataParall
 ``device_ids=[device]`` when world_size > 1.  The one addition is ``gradient_wire_dtype``:
 when set, the DDP buckets are synchronised by ONE fused kernel per bucket (scale by
 1/world, cast to the wire dtype, all-reduce, cast back) instead of the reducer's
-div + all-reduce (+ compress-hook casts).
+div + all-reduce (+ compress-hook casts).  Under ``parallel_strategy="fsdp"`` the same
+option reduce-scatters each FSDP unit's gradient with one fused kernel (scale, cast,
+reduce-scatter, cast back) instead of FSDP's div + fp32 reduce-scatter + div.
 """
 from __future__ import annotations
 
@@ -61,6 +63,34 @@ def b200_grad_hook(wire_dtype: torch.dtype = torch.bfloat16, process_group: Opti
     return hook
 
 
+def b200_fsdp_grad_hook(wire_dtype: torch.dtype = torch.bfloat16,
+                        process_group: Optional[B200ProcessGroup] = None):
+    """FSDP communication hook:
+    ``fsdp_model.register_comm_hook(fsdp_model.process_group, b200_fsdp_grad_hook(torch.bfloat16))``.
+
+    FSDP calls it as ``hook(state, grad, output)`` for the sharded strategies (``grad`` is the padded
+    flat gradient of one FSDP unit, ``output`` its pre-sized shard) and as ``hook(state, grad)`` for
+    ``NO_SHARD``.  Either way the result is the mean gradient, as on FSDP's default path.  For fp32
+    gradients the whole scale-cast-reduce-cast chain is one launch: ``b200_grad_reducescatter`` into
+    ``output``, or ``b200_grad_allreduce`` in place.  ``wait()`` orders FSDP's post-backward stream
+    after it without blocking the host."""
+
+    def hook(state, grad: torch.Tensor, output: Optional[torch.Tensor] = None) -> None:
+        pg = process_group or state or _default_b200_group()
+        n = pg.size()
+        if grad.dtype != torch.float32:
+            # low-precision gradients (mixed-precision parameters): pre-divide and reduce as they are
+            grad.div_(n)
+            work = pg.allreduce([grad]) if output is None else pg._reduce_scatter_base(output, grad)
+            work.wait()
+        elif output is None:
+            pg.grad_allreduce(grad, 1.0 / n, wire_dtype).wait()
+        else:
+            pg.grad_reducescatter(output, grad, 1.0 / n, wire_dtype).wait()
+
+    return hook
+
+
 def prepare_model(model: torch.nn.Module, move_to_device: bool = True, parallel_strategy: Optional[str] = "ddp",
                   parallel_strategy_kwargs: Optional[Dict[str, Any]] = None,
                   gradient_wire_dtype: Optional[torch.dtype] = None) -> torch.nn.Module:
@@ -84,6 +114,9 @@ def prepare_model(model: torch.nn.Module, move_to_device: bool = True, parallel_
             from torch.distributed.fsdp import FullyShardedDataParallel
 
             model = FullyShardedDataParallel(model, **kwargs)
+            if gradient_wire_dtype is not None:
+                # on the root: FSDP gives the hook (with this state) to every unit it wraps
+                model.register_comm_hook(model.process_group, b200_fsdp_grad_hook(gradient_wire_dtype))
         else:
             raise ValueError(f"unknown parallel_strategy {parallel_strategy!r}")
     return model

@@ -3,10 +3,14 @@ GPU, launches replayed from CUDA graphs so host launch overhead does not pollute
 
     python scripts/bw_sweep.py --world 2 [--algos oneshot,twoshot,nvls] [--blocks 0,32,64] \
         [--min 1024 --max 1073741824] [--op allreduce|allgather|reducescatter|broadcast|sendrecv|grad|
-                                            alltoall|alltoall_p2p] [--split uniform|skew|local]
+                                            grad_rs|grad_rs_unfused|alltoall|alltoall_p2p]
+        [--split uniform|skew|local] [--wire bfloat16]
 
 Prints one line per (size, algo, blocks): us per launch, algbw, busbw (nccl-tests convention).
---op takes a comma list; the ops then alternate at every size.  For the all-to-all ops the size
+--op takes a comma list; the ops then alternate at every size.  For the gradient reduce-scatter
+ops the size is one rank's fp32 gradient (all stripes): ``grad_rs`` is the one-launch
+b200_grad_reducescatter, ``grad_rs_unfused`` the composition it replaces ((g * scale).to(wire),
+a reduce-scatter in the wire type, the cast back to fp32).  For the all-to-all ops the size
 is bytes per peer: ``alltoall`` is the one-launch b200_alltoall, ``alltoall_p2p`` the composition
 it replaces (n-1 sends on the rank's stream, n-1 receives on a second stream, a local copy).
 --split skew gives them MoE-like splits instead: rank r sends size >> k bytes to rank r+k (4:2:1:...,
@@ -89,6 +93,13 @@ def alltoall_p2p(c, r, n, outs, ins, side):
     cur.wait_stream(side)
 
 
+def grad_rs_unfused(c, out, grad, wout, scale, wire):
+    """The composition the fused gradient reduce-scatter replaces: scale, cast to the wire type,
+    reduce-scatter in the wire type, cast the shard back into the fp32 output."""
+    c.reducescatter_from(wout, (grad * scale).to(wire), N.SUM)
+    out.copy_(wout)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--world", type=int, default=2)
@@ -104,6 +115,7 @@ def main():
     ap.add_argument("--nvls-ctas", default="-1", help="comma list of CTA counts for the NVLS reduce phase")
     ap.add_argument("--split", default="uniform", choices=["uniform", "skew", "local"],
                     help="all-to-all ops: bytes per peer (see above)")
+    ap.add_argument("--wire", default="bfloat16", help="wire dtype of the grad_rs ops")
     args = ap.parse_args()
     n = args.world
     dtype = getattr(torch, args.dtype)
@@ -156,6 +168,24 @@ def main():
                         ins = [torch.ones(n * numel, dtype=dtype, device=g.device(r)) for r in range(n)]
                         call = lambda c, r: c.reducescatter_from(xs[r], ins[r], N.SUM)  # noqa: E731
                         factor = (n - 1)
+                    elif op in ("grad_rs", "grad_rs_unfused"):
+                        # size = one rank's fp32 gradient (all n stripes); out = its shard
+                        grads = [torch.ones(size // 4, device=g.device(r)) for r in range(n)]
+                        outs = [torch.empty(size // 4 // n, device=g.device(r)) for r in range(n)]
+                        wire = getattr(torch, args.wire)
+                        if op == "grad_rs":
+                            call = lambda c, r: c.grad_reducescatter(outs[r], grads[r], 1.0 / n, wire)  # noqa: E731
+                        else:
+                            wouts = [torch.empty(size // 4 // n, dtype=wire, device=g.device(r)) for r in range(n)]
+                            call = lambda c, r: grad_rs_unfused(c, outs[r], grads[r], wouts[r], 1.0 / n, wire)  # noqa: E731
+                            # run the torch kernels once outside any collective: a kernel's first launch
+                            # may load its module, which waits for the running grids -- and rank 0's
+                            # reduce-scatter grid waits for rank 1, which the host has not issued yet
+                            for r in range(n):
+                                with torch.cuda.device(g.devices[r]):
+                                    (grads[r] * (1.0 / n)).to(wire)
+                                    outs[r].copy_(wouts[r])
+                        factor = (n - 1) / n
                     elif op == "broadcast":
                         call = lambda c, r: c.broadcast(xs[r], 0)  # noqa: E731
                         factor = 1.0
