@@ -211,6 +211,30 @@ int b200_alltoall(b200_comm_t comm, const void *const *ins, const size_t *send_c
 int b200_symm_base(b200_comm_t comm, void **base, size_t *bytes);
 int b200_get(b200_comm_t comm, void *dst, int src_rank, size_t src_heap_offset, size_t nbytes, void *stream);
 
+/* Point-to-point transfer of a tensor LIST as one message (RDT objects, Compiled-Graph channel
+ * messages).  bufs / nbytes are host arrays of ntensors entries; sizes are in BYTES, so one list
+ * may mix dtypes.  Pairwise contract: the receiver passes the same sequence of sizes as the
+ * sender.  A zero-size entry moves nothing, and its pointer may be NULL.  Launches: one per table
+ * of at most B200_P2P_TABLE_MAX non-empty entries, in list order.  Each launch is one message on
+ * the same rings and persistent sequence numbers as b200_send / b200_recv, so it interleaves with
+ * them in stream order.  Wire layout: tensor i starts on a 16-byte unit of the message (units
+ * ustart[i+1] = ustart[i] + ceil(nbytes[i] / 16)); padding travels but is never stored.  Each
+ * side picks its own copy mechanism (ld/st or the bulk-copy unit).  Refused calls (peer out of
+ * range or this rank, ntensors < 0, NULL arrays with ntensors > 0, a NULL pointer with a non-zero
+ * size) launch nothing and return B200_ERR_INVALID.  Counterpart of looping ncclSend / ncclRecv
+ * per tensor (collective_tensor_transport.py). */
+#define B200_P2P_TABLE_MAX 256
+int b200_send_multi(b200_comm_t comm, const void *const *bufs, const size_t *nbytes, int ntensors,
+                    int peer, void *stream);
+int b200_recv_multi(b200_comm_t comm, void *const *bufs, const size_t *nbytes, int ntensors,
+                    int peer, void *stream);
+/* One-sided list get: dsts[i] <- [src_heap_offsets[i], +nbytes[i]) of src_rank's heap, one launch
+ * per table of at most B200_P2P_TABLE_MAX non-empty entries; nothing runs on the owner.  Any range
+ * outside the heap, or a NULL destination with a non-zero size, refuses the whole call before
+ * anything is launched. */
+int b200_get_multi(b200_comm_t comm, void *const *dsts, int src_rank, const size_t *src_heap_offsets,
+                   const size_t *nbytes, int ntensors, void *stream);
+
 /* Fused data-parallel gradient synchronisation (SURVEY K8): for a flat fp32
  * bucket computes grad[i] = sum_r wire(grad_r[i] * scale) in one launch, where
  * wire() is a cast to `wire_dtype` (B200_BF16 / B200_F16 compress the NVLink

@@ -15,7 +15,7 @@ accepts the constructor arguments of torch_tensor_accelerator_channel.py:673-680
 from __future__ import annotations
 
 import uuid
-from typing import Callable, Optional, Tuple
+from typing import Callable, List, Optional, Tuple
 
 import torch
 
@@ -249,6 +249,53 @@ class B200Communicator(Communicator):
         if self._closed:
             raise RayChannelError("B200 group has been destroyed.")
         return buf
+
+    def send_multi(self, bufs: List[torch.Tensor], peer_rank: int) -> None:
+        """``send`` for a list of tensors: one message, one launch per table of tensors."""
+        comm = self._check_open()
+        self._raise_if_failed(comm)
+        try:
+            cur = torch.cuda.current_stream(self._device)
+            if self._send_stream is not cur and self._send_stream.cuda_stream != cur.cuda_stream:
+                self._send_stream.wait_stream(cur)
+                for b in bufs:
+                    b.record_stream(self._send_stream)
+            comm.send_multi(bufs, peer_rank, stream=self._send_stream)
+        except N.B200AbortedError as e:
+            raise RayChannelError(str(e)) from e
+
+    def recv_multi(self, metas: List[Tuple[Tuple[int], torch.dtype]], peer_rank: int,
+                   allocator: Optional[TorchTensorAllocator] = None) -> List[torch.Tensor]:
+        """``recv`` for a list of (shape, dtype): the peer's ``send_multi`` in one message.  Every
+        returned tensor carries the ``_b200_ready`` event of the receive."""
+        comm = self._check_open()
+        assert allocator is not None, "B200 group requires a tensor allocator"
+        self._raise_if_failed(comm)
+        bufs = [allocator(shape, dtype) for shape, dtype in metas]
+        try:
+            cur = torch.cuda.current_stream(self._device)
+            same = self._recv_stream is cur or self._recv_stream.cuda_stream == cur.cuda_stream
+            if not same:
+                self._recv_stream.wait_stream(cur)  # the allocations may recycle memory still in use on `cur`
+                for b in bufs:
+                    b.record_stream(self._recv_stream)
+            comm.recv_multi(bufs, peer_rank, stream=self._recv_stream)
+            if self._host_sync:
+                self._recv_stream.synchronize()
+                self._raise_if_failed(comm)
+            else:
+                ev = torch.cuda.Event()
+                ev.record(self._recv_stream)
+                if not same:
+                    cur.wait_event(ev)
+                for b in bufs:
+                    b._b200_ready = ev  # noqa: SLF001
+                self._last_recv_event = ev
+        except N.B200AbortedError as e:
+            raise RayChannelError(str(e)) from e
+        if self._closed:
+            raise RayChannelError("B200 group has been destroyed.")
+        return bufs
 
     def wait(self, tensor: Optional[torch.Tensor] = None) -> None:
         """Block the host until ``tensor`` (default: the most recent recv) has arrived, then raise

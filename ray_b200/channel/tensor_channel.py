@@ -14,7 +14,8 @@ cudaMemcpy: the kernels read / write the pinned buffer through unified addressin
 dynamic-shape message costs one extra small kernel and one event wait on the reader instead of
 a pickle + futex round trip, and the channel needs no second transport.  When the channel spans
 the whole group and has several readers the payload is one broadcast instead of a send per
-reader.
+reader; otherwise it is one list send per reader (``send_multi`` / ``recv_multi``) instead of one
+send per tensor.
 """
 from __future__ import annotations
 
@@ -103,6 +104,9 @@ class TorchTensorAcceleratorChannel:
         world = communicator.get_world_size()
         self._use_broadcast = (len(self._reader_ranks) > 1 and hasattr(communicator, "broadcast") and
                                set(self._reader_ranks) | {writer_rank} == set(range(world)))
+        # Point-to-point path: a communicator with list send / recv (B200Communicator) moves the
+        # payload of a message as one message per reader instead of one per tensor.
+        self._send_multi = hasattr(communicator, "send_multi") and hasattr(communicator, "recv_multi")
         # pinned allocations synchronise the device implicitly: do it now, not in the middle of a
         # write()/read() while a peer's kernel may be waiting for ours
         if me is not None and not static_shape and torch.cuda.is_available():
@@ -158,8 +162,11 @@ class TorchTensorAcceleratorChannel:
                 self._comm.broadcast(t, self._writer_rank)
             return
         for rank in self._reader_ranks:
-            for t in contig:
-                self._comm.send(t, rank)
+            if self._send_multi:
+                self._comm.send_multi(contig, rank)  # the whole message in one launch
+            else:
+                for t in contig:
+                    self._comm.send(t, rank)
 
     # ------------------------------------------------------------------ reader
     def read(self, timeout: Optional[float] = None):
@@ -188,6 +195,8 @@ class TorchTensorAcceleratorChannel:
                 b = self._allocator(shape, dtype)
                 self._comm.broadcast(b, self._writer_rank)
                 bufs.append(b)
+        elif self._send_multi:
+            bufs = self._comm.recv_multi(meta, self._writer_rank, self._allocator)
         else:
             bufs = [self._comm.recv(shape, dtype, self._writer_rank, self._allocator) for shape, dtype in meta]
         if self._direct_return:

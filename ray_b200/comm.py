@@ -50,6 +50,17 @@ def _check_cuda_contiguous(t: torch.Tensor, what: str = "tensor") -> None:
         raise RuntimeError(f"{what} must be contiguous")
 
 
+def _tensor_list(tensors: Sequence[torch.Tensor]):
+    """(pointer array, byte-size array) of a list of contiguous CUDA tensors."""
+    ptrs = (ctypes.c_void_p * max(len(tensors), 1))()
+    sizes = (ctypes.c_size_t * max(len(tensors), 1))()
+    for i, t in enumerate(tensors):
+        _check_cuda_contiguous(t, f"tensor {i}")
+        ptrs[i] = t.data_ptr()
+        sizes[i] = t.numel() * t.element_size()
+    return ptrs, sizes
+
+
 class SymmetricTensorHolder:
     """Exposes a slice of the symmetric heap through __cuda_array_interface__."""
 
@@ -337,6 +348,24 @@ class B200Comm:
         if st:
             N.check(st)
 
+    def send_multi(self, tensors: Sequence[torch.Tensor], peer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Send a list of tensors (any dtypes) as one message: one launch per ``N.P2P_TABLE_MAX``
+        non-empty tensors instead of one per tensor.  The peer's ``recv_multi`` must pass tensors
+        of the same byte sizes in the same order."""
+        ptrs, sizes = _tensor_list(tensors)
+        if not tensors:
+            return
+        N.check(self._lib.b200_send_multi(self._h, ptrs, sizes, len(tensors), int(peer),
+                                          stream.cuda_stream if stream is not None else self._stream()))
+
+    def recv_multi(self, tensors: Sequence[torch.Tensor], peer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Receive what the peer's ``send_multi`` sent into ``tensors`` (same byte sizes, same order)."""
+        ptrs, sizes = _tensor_list(tensors)
+        if not tensors:
+            return
+        N.check(self._lib.b200_recv_multi(self._h, ptrs, sizes, len(tensors), int(peer),
+                                          stream.cuda_stream if stream is not None else self._stream()))
+
     def send_ptr(self, ptr: int, nbytes: int, peer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
         """send() from a raw device-visible address (e.g. pinned host memory under unified
         addressing: the Compiled-Graph channel keeps its metadata header there)."""
@@ -376,6 +405,19 @@ class B200Comm:
         N.check(self._lib.b200_get(self._h, dst.data_ptr(), int(src_rank), int(src_heap_offset),
                                    dst.numel() * dst.element_size(),
                                    stream.cuda_stream if stream is not None else self._stream()))
+
+    def get_multi(self, dsts: Sequence[torch.Tensor], src_rank: int, src_heap_offsets: Sequence[int],
+                  stream: Optional[torch.cuda.Stream] = None) -> None:
+        """``get`` for a list: ``dsts[i]`` receives ``dsts[i].nbytes`` bytes from ``src_heap_offsets[i]``
+        of ``src_rank``'s heap, one launch per ``N.P2P_TABLE_MAX`` non-empty tensors."""
+        if len(dsts) != len(src_heap_offsets):
+            raise ValueError(f"get_multi got {len(dsts)} destination tensors but {len(src_heap_offsets)} offsets")
+        ptrs, sizes = _tensor_list(dsts)
+        if not dsts:
+            return
+        offs = (ctypes.c_size_t * len(dsts))(*[int(o) for o in src_heap_offsets])
+        N.check(self._lib.b200_get_multi(self._h, ptrs, int(src_rank), offs, sizes, len(dsts),
+                                         stream.cuda_stream if stream is not None else self._stream()))
 
     def grad_allreduce(self, grad: torch.Tensor, scale: float, wire_dtype: torch.dtype = torch.bfloat16) -> None:
         """Fused ``grad = sum_r wire(grad_r * scale)`` on a flat fp32 bucket (SURVEY K8)."""

@@ -26,7 +26,8 @@
 //                     system-scope fence.
 // Both are thin wrappers around p2p_ldst_ring / p2p_bulk_ring (one CTA's share of a message), which
 // alltoall_kernel also runs: all 2(n-1) transfers of an all-to-all as roles of one grid, each role
-// picking its own copy mechanism.
+// picking its own copy mechanism.  The same two functions move a table of tensors as one message
+// (p2p_table_kernel / p2p_bulk_table_kernel: b200_send_multi / b200_recv_multi).
 #include <type_traits>
 
 #include "bulk_copy.cuh"
@@ -48,16 +49,73 @@ __device__ __forceinline__ bool cta_wait_flag(const DevComm &c, const uint32_t *
   return ok != 0;
 }
 
+// ---------------------------------------------------------------------------
+// Where the bytes of a message live: one contiguous buffer (char *), or a table of tensors
+// (b200_send_multi / b200_recv_multi).  A table's tensors form ONE packed message: tensor i
+// occupies 16-byte units [ustart[i], ustart[i+1]) with ustart[i+1] = ustart[i] + ceil(nbytes[i] / 16),
+// so no unit mixes two tensors.  The padding of a tensor's last unit travels on the wire (zeros)
+// and is never stored.  Entries are non-empty: the host drops zero-size ones on both sides.
+// ---------------------------------------------------------------------------
+struct P2PTable {
+  int count;
+  char *ptr[kP2PTableMax];
+  unsigned long long nbytes[kP2PTableMax];
+  unsigned long long ustart[kP2PTableMax + 1];
+};
+
+struct P2PTableArgs {
+  P2PTable t;
+  size_t nbytes;  // bytes on the wire: 16 * ustart[count]
+  size_t chunk;
+  int peer;
+};
+
+// the entry that owns unit u of a table's packed message (ustart strictly increasing)
+__device__ __forceinline__ int table_entry(const unsigned long long *start, int count, size_t u) {
+  int lo = 0, hi = count - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (start[mid] <= u) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// unit u (of the whole message) of a table, loaded / stored like a unit of a user tensor
+__device__ __forceinline__ uint4 table_load_unit(const P2PTable &t, size_t u) {
+  const int i = table_entry(t.ustart, t.count, u);
+  return load_user_unit(t.ptr[i], u - t.ustart[i], make_units(t.nbytes[i]), is_aligned16(t.ptr[i]));
+}
+__device__ __forceinline__ void table_store_unit(const P2PTable &t, size_t u, uint4 v) {
+  const int i = table_entry(t.ustart, t.count, u);
+  store_user_unit(t.ptr[i], u - t.ustart[i], make_units(t.nbytes[i]), is_aligned16(t.ptr[i]), v);
+}
+
+// unit u of the chunk that starts at byte lo of the message
+__device__ __forceinline__ uint4 msg_load_unit(char *buf, size_t lo, size_t u, const Units &un, bool al) {
+  return load_user_unit(buf + lo, u, un, al);
+}
+__device__ __forceinline__ uint4 msg_load_unit(const P2PTable *t, size_t lo, size_t u, const Units &, bool) {
+  return table_load_unit(*t, (lo >> 4) + u);
+}
+__device__ __forceinline__ void msg_store_unit(char *buf, size_t lo, size_t u, const Units &un, bool al, uint4 v) {
+  store_user_unit(buf + lo, u, un, al, v);
+}
+__device__ __forceinline__ void msg_store_unit(const P2PTable *t, size_t lo, size_t u, const Units &, bool, uint4 v) {
+  table_store_unit(*t, (lo >> 4) + u, v);
+}
+
 // One CTA's share of a message: chunks b, b + G, b + 2G, ... over sub-ring b, moved with 16-byte
-// ld/st by all kThreads threads.  Both sides of a pair call it with the same (G, chunk).
-template <bool SEND>
-__device__ __forceinline__ void p2p_ldst_ring(const DevComm &c, int peer, int b, int G, char *buf, size_t nbytes,
+// ld/st by all kThreads threads.  Both sides of a pair call it with the same (G, chunk).  `msg` is
+// a buffer (char *) or a table (const P2PTable *); a table's chunks are whole 16-byte units.
+template <bool SEND, typename Msg>
+__device__ __forceinline__ void p2p_ldst_ring(const DevComm &c, int peer, int b, int G, Msg msg, size_t nbytes,
                                               size_t chunk) {
   const int me = c.rank;
   const size_t ring_bytes = c.inbox_bytes / kP2PRings;
   const size_t slot_bytes = ring_bytes / kP2PSlots;
   const size_t nchunks = (nbytes + chunk - 1) / chunk;
-  const bool al = is_aligned16(buf);
+  const bool al = is_aligned16(msg);
 
   uint32_t *seq_word = SEND ? &c.st->send_seq[peer][b] : &c.st->recv_seq[peer][b];
   uint32_t seq = *seq_word;
@@ -78,7 +136,6 @@ __device__ __forceinline__ void p2p_ldst_ring(const DevComm &c, int peer, int b,
     const size_t U = un.total();
     const uint32_t slot = seq % kP2PSlots;
     char *slot_ptr = ring + size_t(slot) * slot_bytes;
-    char *user = buf + lo;
     if (SEND) {
       // slot free once the receiver consumed chunk (seq - kP2PSlots)
       if (!cta_wait_flag(c, ack, seq + 1u - kP2PSlots)) break;
@@ -89,7 +146,7 @@ __device__ __forceinline__ void p2p_ldst_ring(const DevComm &c, int peer, int b,
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           const size_t u = u0 + size_t(k) * kThreads;
-          if (u < U) v[k] = load_user_unit(user, u, un, al);
+          if (u < U) v[k] = msg_load_unit(msg, lo, u, un, al);
         }
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
@@ -111,7 +168,7 @@ __device__ __forceinline__ void p2p_ldst_ring(const DevComm &c, int peer, int b,
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           const size_t u = u0 + size_t(k) * kThreads;
-          if (u < U) store_user_unit(user, u, un, al, v[k]);
+          if (u < U) msg_store_unit(msg, lo, u, un, al, v[k]);
         }
       }
       __syncthreads();
@@ -131,12 +188,77 @@ __global__ void __launch_bounds__(kThreads, 1) p2p_kernel(DevComm c, P2PArgs a) 
 // ---------------------------------------------------------------------------
 // bulk-copy variant: same rings, same flags, same sequence numbers
 // ---------------------------------------------------------------------------
-// The same share of a message moved by the bulk-copy unit; `dyn_smem` holds kBulkSmemBytes.  `buf`
-// must be 16-byte aligned and `nbytes` a multiple of 16.  Only threads 0 and 32 drive the transfer;
-// warps 2.. run side(thread, nthreads) meanwhile (the all-to-all gives them its own-segment copy).
-template <bool SEND, typename SideFn>
-__device__ __forceinline__ void p2p_bulk_ring(const DevComm &c, int peer, int b, int G, char *buf, size_t nbytes,
+// Bulk segments of one CTA's chunks of a table: a chunk that spans several tensors is one segment
+// per (chunk, tensor) pair.  The segment engine asks for segments through three cursors (load, store,
+// completion), each in increasing order; `at` keeps one position per cursor and walks forward from
+// the nearest one at or below the request, so a lookup costs O(1) amortised -- per segment, never
+// per tile.
+struct TableSegs {
+  struct Pos {
+    uint32_t seg;  // segment index within this CTA
+    uint32_t q;    // chunk of this CTA
+    int t;         // table entry
+  };
+  const P2PTable &tb;
+  size_t b, G, cu, tu;  // CTA, CTAs, units per chunk, units of the message
+  Pos p0, p1, p2;       // named, not an array: the copy thread keeps them in registers
+
+  __device__ TableSegs(const P2PTable &t, int b_, int G_, size_t chunk)
+      : tb(t), b(size_t(b_)), G(size_t(G_)), cu(chunk >> 4), tu(t.ustart[t.count]) {
+    p0 = p1 = p2 = start();
+  }
+  __device__ Pos start() const { return Pos{0, 0, table_entry(tb.ustart, tb.count, lo(0))}; }
+  __device__ size_t lo(uint32_t q) const { return (b + size_t(q) * G) * cu; }
+  __device__ size_t hi(uint32_t q) const { return lo(q) + cu < tu ? lo(q) + cu : tu; }
+  // segments of the first nq chunks of this CTA
+  __device__ uint32_t count(uint32_t nq) const {
+    uint32_t n = 0;
+    for (uint32_t q = 0; q < nq; ++q)
+      n += uint32_t(table_entry(tb.ustart, tb.count, hi(q) - 1) - table_entry(tb.ustart, tb.count, lo(q)) + 1);
+    return n;
+  }
+  __device__ Pos at(uint32_t i) {
+    int k = -1;
+    uint32_t best = 0;
+    if (p0.seg <= i) k = 0, best = p0.seg;
+    if (p1.seg <= i && (k < 0 || p1.seg > best)) k = 1, best = p1.seg;
+    if (p2.seg <= i && (k < 0 || p2.seg > best)) k = 2;
+    Pos p = k == 0 ? p0 : k == 1 ? p1 : k == 2 ? p2 : start();
+    while (p.seg < i) {
+      ++p.seg;
+      if (tb.ustart[p.t + 1] < hi(p.q)) {
+        ++p.t;
+      } else {
+        ++p.q;
+        p.t = table_entry(tb.ustart, tb.count, lo(p.q));
+      }
+    }
+    if (k == 1) p1 = p;
+    else if (k == 2) p2 = p;
+    else p0 = p;
+    return p;
+  }
+  __device__ bool opens_chunk(const Pos &p) const { return tb.ustart[p.t] <= lo(p.q); }
+  __device__ bool closes_chunk(const Pos &p) const { return tb.ustart[p.t + 1] >= hi(p.q); }
+  // (user bytes, offset in the chunk, bytes) of segment p: every tensor of a bulk table is whole units
+  __device__ BulkSeg seg(const Pos &p, char *chunk_slot, bool send) const {
+    const size_t s = tb.ustart[p.t], e = tb.ustart[p.t + 1];
+    const size_t ulo = s > lo(p.q) ? s : lo(p.q), uhi = e < hi(p.q) ? e : hi(p.q);
+    char *user = tb.ptr[p.t] + ((ulo - s) << 4);
+    char *slot = chunk_slot + ((ulo - lo(p.q)) << 4);
+    const uint32_t len = uint32_t((uhi - ulo) << 4);
+    return send ? BulkSeg{user, slot, len} : BulkSeg{slot, user, len};
+  }
+};
+
+// The same share of a message moved by the bulk-copy unit; `dyn_smem` holds kBulkSmemBytes.  A
+// buffer `msg` must be 16-byte aligned and `nbytes` a multiple of 16; so must every tensor of a
+// table.  Only threads 0 and 32 drive the transfer; warps 2.. run side(thread, nthreads) meanwhile
+// (the all-to-all gives them its own-segment copy).
+template <bool SEND, typename Msg, typename SideFn>
+__device__ __forceinline__ void p2p_bulk_ring(const DevComm &c, int peer, int b, int G, Msg msg, size_t nbytes,
                                               size_t chunk, char *dyn_smem, SideFn side) {
+  constexpr bool kTable = std::is_same<Msg, const P2PTable *>::value;
   __shared__ volatile uint32_t mailbox;  // chunks of this CTA whose bytes have all been moved
   __shared__ volatile int stop;
   const int me = c.rank;
@@ -161,13 +283,7 @@ __device__ __forceinline__ void p2p_bulk_ring(const DevComm &c, int peer, int b,
 
   const uint32_t nq32 = uint32_t(nq);
   if (threadIdx.x == 0 && nq > 0) {
-    // ---- copy thread: one segment per chunk ---------------------------------------------------
-    auto seg = [&](uint32_t q) {
-      const size_t lo = (size_t(b) + size_t(q) * size_t(G)) * chunk;
-      const uint32_t len = uint32_t((nbytes - lo) < chunk ? (nbytes - lo) : chunk);
-      char *slot = ring + size_t((seq0 + q) % kP2PSlots) * slot_bytes;
-      return SEND ? BulkSeg{buf + lo, slot, len} : BulkSeg{slot, buf + lo, len};
-    };
+    // ---- copy thread: one segment per chunk (per chunk and tensor for a table) ------------------
     auto gate = [&](uint32_t q, bool block) {
       const uint32_t seq = seq0 + q;
       // sender: the slot was consumed (ack in MY pad); receiver: the chunk landed (ready in MY pad)
@@ -186,8 +302,37 @@ __device__ __forceinline__ void p2p_bulk_ring(const DevComm &c, int peer, int b,
       mailbox = q + 1;
     };
     // the sender's stores cross NVLink, the receiver's stay in local HBM
-    const bool ok = SEND ? bulk_copy_segments<BulkRemote>(br, nq32, seg, gate, done)
-                         : bulk_copy_segments<BulkLocal>(br, nq32, seg, gate, done);
+    auto copy = [&](uint32_t nsegs, auto seg, auto seg_gate, auto seg_done) {
+      return SEND ? bulk_copy_segments<BulkRemote>(br, nsegs, seg, seg_gate, seg_done)
+                  : bulk_copy_segments<BulkLocal>(br, nsegs, seg, seg_gate, seg_done);
+    };
+    bool ok;
+    if constexpr (kTable) {
+      // a chunk's gate runs before its first segment, its done after its last
+      TableSegs ts(*msg, b, G, chunk);
+      ok = copy(
+          ts.count(nq32),
+          [&](uint32_t i) {
+            const TableSegs::Pos p = ts.at(i);
+            return ts.seg(p, ring + size_t((seq0 + p.q) % kP2PSlots) * slot_bytes, SEND);
+          },
+          [&](uint32_t i, bool block) {
+            const TableSegs::Pos p = ts.at(i);
+            return ts.opens_chunk(p) ? gate(p.q, block) : 1;
+          },
+          [&](uint32_t i) {
+            const TableSegs::Pos p = ts.at(i);
+            if (ts.closes_chunk(p)) done(p.q);
+          });
+    } else {
+      auto seg = [&](uint32_t q) {
+        const size_t lo = (size_t(b) + size_t(q) * size_t(G)) * chunk;
+        const uint32_t len = uint32_t((nbytes - lo) < chunk ? (nbytes - lo) : chunk);
+        char *slot = ring + size_t((seq0 + q) % kP2PSlots) * slot_bytes;
+        return SEND ? BulkSeg{msg + lo, slot, len} : BulkSeg{slot, msg + lo, len};
+      };
+      ok = copy(nq32, seg, gate, done);
+    }
     if (!ok) stop = 1;
   } else if (threadIdx.x == 32 && nq > 0) {
     // ---- flag thread: publishes "ready" (sender) / "ack" (receiver) for completed chunks ------
@@ -219,6 +364,21 @@ template <bool SEND>
 __global__ void __launch_bounds__(kThreads, 1) p2p_bulk_kernel(DevComm c, P2PArgs a) {
   extern __shared__ __align__(128) char dyn_smem[];
   p2p_bulk_ring<SEND>(c, a.peer, blockIdx.x, gridDim.x, a.buf, a.nbytes, a.chunk, dyn_smem, [](int, int) {});
+}
+
+// A table of tensors as one message (b200_send_multi / b200_recv_multi): the same rings, flags and
+// sequence numbers, so it interleaves with b200_send / b200_recv in stream order.  The table stays
+// in parameter space (__grid_constant__), indexed in place.
+template <bool SEND>
+__global__ void __launch_bounds__(kThreads, 1) p2p_table_kernel(DevComm c, const __grid_constant__ P2PTableArgs a) {
+  p2p_ldst_ring<SEND>(c, a.peer, blockIdx.x, gridDim.x, &a.t, a.nbytes, a.chunk);
+}
+
+template <bool SEND>
+__global__ void __launch_bounds__(kThreads, 1)
+    p2p_bulk_table_kernel(DevComm c, const __grid_constant__ P2PTableArgs a) {
+  extern __shared__ __align__(128) char dyn_smem[];
+  p2p_bulk_ring<SEND>(c, a.peer, blockIdx.x, gridDim.x, &a.t, a.nbytes, a.chunk, dyn_smem, [](int, int) {});
 }
 
 // ---------------------------------------------------------------------------
@@ -330,21 +490,49 @@ struct GetArgs {
   size_t seg_bytes;
 };
 
-__global__ void __launch_bounds__(kThreads, 1) get_bulk_kernel(GetArgs a) {
-  extern __shared__ __align__(128) char dyn_smem[];
+// A list of gets in one launch (b200_get_multi).  start[] is a prefix over the entries: their first
+// 16-byte unit for the ld/st kernel, their first bulk segment for the bulk kernel.
+struct GetTable {
+  int count;
+  const char *src[kP2PTableMax];  // peer mapping of the owner's heap + offset
+  char *dst[kP2PTableMax];
+  unsigned long long nbytes[kP2PTableMax];
+  unsigned long long start[kP2PTableMax + 1];
+  size_t seg_bytes;
+};
+
+// Segments b, b + G, b + 2G, ... of nseg() segments of a get (seg_of(k): global segment k), pulled
+// by thread 0
+template <typename NsegFn, typename SegOf>
+__device__ __forceinline__ void get_bulk_segments(char *dyn_smem, NsegFn nsegs, SegOf seg_of) {
   const BulkRing br = bulk_ring_init(dyn_smem);
   if (threadIdx.x != 0) return;
-  const size_t nseg = (a.nbytes + a.seg_bytes - 1) / a.seg_bytes;
+  const size_t nseg = nsegs();
   const uint32_t b = blockIdx.x, G = gridDim.x;
   const uint32_t mine = nseg > b ? uint32_t((nseg - 1 - b) / G + 1) : 0;
   bulk_copy_segments<BulkPull>(
-      br, mine,
-      [&](uint32_t i) {
-        const size_t lo = (size_t(b) + size_t(i) * G) * a.seg_bytes;
-        const uint32_t len = uint32_t((a.nbytes - lo) < a.seg_bytes ? (a.nbytes - lo) : a.seg_bytes);
-        return BulkSeg{a.src + lo, a.dst + lo, len};
-      },
-      [&](uint32_t, bool) { return 1; }, [&](uint32_t) {});
+      br, mine, [&](uint32_t i) { return seg_of(size_t(b) + size_t(i) * G); }, [&](uint32_t, bool) { return 1; },
+      [&](uint32_t) {});
+}
+
+__global__ void __launch_bounds__(kThreads, 1) get_bulk_kernel(GetArgs a) {
+  extern __shared__ __align__(128) char dyn_smem[];
+  get_bulk_segments(dyn_smem, [&] { return (a.nbytes + a.seg_bytes - 1) / a.seg_bytes; }, [&](size_t k) {
+    const size_t lo = k * a.seg_bytes;
+    const uint32_t len = uint32_t((a.nbytes - lo) < a.seg_bytes ? (a.nbytes - lo) : a.seg_bytes);
+    return BulkSeg{a.src + lo, a.dst + lo, len};
+  });
+}
+
+// entry i is aligned and whole units on both ends (host check); its segments are [start[i], start[i+1])
+__global__ void __launch_bounds__(kThreads, 1) get_bulk_table_kernel(const __grid_constant__ GetTable a) {
+  extern __shared__ __align__(128) char dyn_smem[];
+  get_bulk_segments(dyn_smem, [&] { return size_t(a.start[a.count]); }, [&](size_t k) {
+    const int i = table_entry(a.start, a.count, k);
+    const size_t lo = (k - a.start[i]) * a.seg_bytes;
+    const uint32_t len = uint32_t((a.nbytes[i] - lo) < a.seg_bytes ? (a.nbytes[i] - lo) : a.seg_bytes);
+    return BulkSeg{a.src[i] + lo, a.dst[i] + lo, len};
+  });
 }
 
 __global__ void __launch_bounds__(kThreads) get_ldst_kernel(GetArgs a) {
@@ -356,6 +544,20 @@ __global__ void __launch_bounds__(kThreads) get_ldst_kernel(GetArgs a) {
     if (sal && u < un.full) v = ld_peer(a.src + (u << 4));
     else v = load_user_unit(a.src, u, un, false);
     store_user_unit(a.dst, u, un, dal, v);
+  }
+}
+
+// unit u of the packed list is unit u - start[i] of entry i; alignment is taken per entry
+__global__ void __launch_bounds__(kThreads) get_ldst_table_kernel(const __grid_constant__ GetTable a) {
+  const size_t U = a.start[a.count];
+  for (size_t u = size_t(blockIdx.x) * kThreads + threadIdx.x; u < U; u += size_t(gridDim.x) * kThreads) {
+    const int i = table_entry(a.start, a.count, u);
+    const Units un = make_units(a.nbytes[i]);
+    const size_t w = u - a.start[i];
+    uint4 v;
+    if (is_aligned16(a.src[i]) && w < un.full) v = ld_peer(a.src[i] + (w << 4));
+    else v = load_user_unit(a.src[i], w, un, false);
+    store_user_unit(a.dst[i], w, un, is_aligned16(a.dst[i]), v);
   }
 }
 
@@ -385,6 +587,88 @@ static int p2p_common(b200_comm *c, void *buf, size_t nbytes, int peer, cudaStre
   return B200_OK;
 }
 
+// ---- tensor lists -----------------------------------------------------------------------------
+
+// ntensors and the host arrays of a list entry point
+static int check_list(int ntensors, bool arrays) {
+  if (ntensors < 0) {
+    set_error("ntensors %d is negative", ntensors);
+    return B200_ERR_INVALID;
+  }
+  if (ntensors > 0 && !arrays) {
+    set_error("null argument array");
+    return B200_ERR_INVALID;
+  }
+  return B200_OK;
+}
+
+static int check_list_ptrs(const void *const *ptrs, const size_t *nbytes, int ntensors) {
+  for (int i = 0; i < ntensors; ++i) {
+    if (nbytes[i] && !ptrs[i]) {
+      set_error("tensor %d is null but has %zu bytes", i, nbytes[i]);
+      return B200_ERR_INVALID;
+    }
+  }
+  return B200_OK;
+}
+
+// Runs launch(lo, hi) over [0, ntensors) cut into runs of at most kP2PTableMax non-empty entries, in
+// list order.  The cut depends on the size list alone, so sender and receiver cut alike.
+template <typename Fn>
+static int for_each_table(const size_t *nbytes, int ntensors, Fn launch) {
+  int lo = 0, count = 0;
+  for (int i = 0; i < ntensors; ++i) {
+    if (!nbytes[i]) continue;
+    if (count == kP2PTableMax) {
+      if (int rc = launch(lo, i)) return rc;
+      lo = i;
+      count = 0;
+    }
+    ++count;
+  }
+  return count ? launch(lo, ntensors) : B200_OK;
+}
+
+static int p2p_multi_common(b200_comm *c, void *const *bufs, const size_t *nbytes, int ntensors, int peer,
+                            cudaStream_t stream, bool send) {
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_rank(c, peer, "peer"))) return rc;
+  if (peer == c->rank) {
+    set_error("peer rank %d is this rank", peer);
+    return B200_ERR_INVALID;
+  }
+  if ((rc = check_list(ntensors, bufs && nbytes)) || (rc = check_list_ptrs(bufs, nbytes, ntensors))) return rc;
+  if (ntensors == 0) return B200_OK;
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  return for_each_table(nbytes, ntensors, [&](int lo, int hi) -> int {
+    P2PTableArgs a{};
+    bool whole_aligned = true;
+    for (int i = lo; i < hi; ++i) {
+      if (!nbytes[i]) continue;
+      const int k = a.t.count++;
+      a.t.ptr[k] = static_cast<char *>(bufs[i]);
+      a.t.nbytes[k] = nbytes[i];
+      a.t.ustart[k + 1] = a.t.ustart[k] + (nbytes[i] + 15) / 16;
+      whole_aligned = whole_aligned && is_aligned16(bufs[i]) && (nbytes[i] & 15) == 0;
+    }
+    a.nbytes = size_t(a.t.ustart[a.t.count]) * 16;
+    const P2PPlan p = p2p_table_plan(c, a.nbytes, a.t.count, whole_aligned);
+    a.chunk = p.chunk;
+    a.peer = peer;
+    if (p.bulk) {
+      auto k = send ? p2p_bulk_table_kernel<true> : p2p_bulk_table_kernel<false>;
+      if (int rc2 = set_dyn_smem(c->device, reinterpret_cast<const void *>(k))) return rc2;
+      k<<<p.rings, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a);
+    } else if (send) {
+      p2p_table_kernel<true><<<p.rings, kThreads, 0, stream>>>(c->dev(), a);
+    } else {
+      p2p_table_kernel<false><<<p.rings, kThreads, 0, stream>>>(c->dev(), a);
+    }
+    B200_LAUNCH_CHECK(c);
+    return B200_OK;
+  });
+}
+
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
 const void *p2p_module_anchor() { return reinterpret_cast<const void *>(&get_bulk_kernel); }
 
@@ -398,6 +682,17 @@ extern "C" int b200_send(b200_comm_t c, const void *buf, size_t nbytes, int peer
 
 extern "C" int b200_recv(b200_comm_t c, void *buf, size_t nbytes, int peer, void *stream) {
   return p2p_common(c, buf, nbytes, peer, static_cast<cudaStream_t>(stream), false);
+}
+
+extern "C" int b200_send_multi(b200_comm_t c, const void *const *bufs, const size_t *nbytes, int ntensors, int peer,
+                               void *stream) {
+  return p2p_multi_common(c, const_cast<void *const *>(bufs), nbytes, ntensors, peer,
+                          static_cast<cudaStream_t>(stream), true);
+}
+
+extern "C" int b200_recv_multi(b200_comm_t c, void *const *bufs, const size_t *nbytes, int ntensors, int peer,
+                               void *stream) {
+  return p2p_multi_common(c, bufs, nbytes, ntensors, peer, static_cast<cudaStream_t>(stream), false);
 }
 
 extern "C" int b200_alltoall(b200_comm_t c, const void *const *ins, const size_t *send_counts, void *const *outs,
@@ -532,4 +827,53 @@ extern "C" int b200_get(b200_comm_t c, void *dst, int src_rank, size_t src_heap_
   }
   B200_LAUNCH_CHECK(c);
   return B200_OK;
+}
+
+extern "C" int b200_get_multi(b200_comm_t c, void *const *dsts, int src_rank, const size_t *src_heap_offsets,
+                              const size_t *nbytes, int ntensors, void *stream_) {
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_rank(c, src_rank, "source")) ||
+      (rc = check_list(ntensors, dsts && src_heap_offsets && nbytes)))
+    return rc;
+  for (int i = 0; i < ntensors; ++i) {
+    if (src_heap_offsets[i] > c->heap_bytes || nbytes[i] > c->heap_bytes - src_heap_offsets[i]) {
+      set_error("tensor %d: [%zu, %zu) is outside the %zu-byte symmetric heap", i, src_heap_offsets[i],
+                src_heap_offsets[i] + nbytes[i], c->heap_bytes);
+      return B200_ERR_INVALID;
+    }
+  }
+  if ((rc = check_list_ptrs(dsts, nbytes, ntensors))) return rc;
+  if (ntensors == 0) return B200_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  const char *heap = reinterpret_cast<const char *>(c->data.va[src_rank]) + 2 * c->staging_bytes;
+  return for_each_table(nbytes, ntensors, [&](int lo, int hi) -> int {
+    GetTable a{};
+    a.seg_bytes = kGetSegBytes;
+    bool whole_aligned = true;
+    size_t total = 0;
+    for (int i = lo; i < hi; ++i) {
+      if (!nbytes[i]) continue;
+      const int k = a.count++;
+      a.src[k] = heap + src_heap_offsets[i];
+      a.dst[k] = static_cast<char *>(dsts[i]);
+      a.nbytes[k] = nbytes[i];
+      total += nbytes[i];
+      whole_aligned = whole_aligned && is_aligned16(a.src[k]) && is_aligned16(a.dst[k]) && (nbytes[i] & 15) == 0;
+    }
+    const bool bulk = get_table_bulk(total, a.count, whole_aligned);
+    const size_t step = bulk ? a.seg_bytes : 16;  // start[] counts segments or 16-byte units
+    for (int k = 0; k < a.count; ++k) a.start[k + 1] = a.start[k] + (a.nbytes[k] + step - 1) / step;
+    const size_t n = a.start[a.count];
+    if (bulk) {
+      const int g = int(n < 16 ? n : 16);
+      if (int rc2 = set_dyn_smem(c->device, reinterpret_cast<const void *>(get_bulk_table_kernel))) return rc2;
+      get_bulk_table_kernel<<<g, kThreads, kBulkSmemBytes, stream>>>(a);
+    } else {
+      const int g = int((n + kThreads - 1) / kThreads < 32 ? (n + kThreads - 1) / kThreads : 32);
+      get_ldst_table_kernel<<<g, kThreads, 0, stream>>>(a);
+    }
+    B200_LAUNCH_CHECK(c);
+    return B200_OK;
+  });
 }

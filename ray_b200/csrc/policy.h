@@ -204,6 +204,26 @@ inline P2PPlan p2p_plan(const b200_comm *c, const void *buf, size_t nbytes) {
   return p;
 }
 
+// Tensor lists (b200_send_multi / b200_recv_multi / b200_get_multi) travel as tables of at most
+// kP2PTableMax non-empty entries, one launch per table.  The table is a __grid_constant__ kernel
+// parameter: CUDA >= 12.1 allows 32764 bytes of parameters on sm_90, and 256 entries take about
+// 6 KiB (send / recv) or 8 KiB (get).  What a parameter block that large costs per launch has not
+// been measured.
+constexpr int kP2PTableMax = B200_P2P_TABLE_MAX;
+
+// A table is ONE message of 16 * (sum of ceil(nbytes[i] / 16)) bytes: the protocol (chunk, rings)
+// is p2p_plan's for that packed size, a pure function of the size list.  This side moves its bytes
+// with the bulk-copy unit when p2p_plan would for the packed size, every tensor of its table is
+// 16-byte aligned and whole units, and the tensors average at least kP2PTableBulkMinAvg bytes: every
+// (chunk, tensor) piece is a bulk segment with its own set-up, which small tensors do not repay.
+// The 32 KiB threshold mirrors B200_PARAM_P2P_BULK_MIN_CHUNK's default; it was not tuned.
+constexpr size_t kP2PTableBulkMinAvg = size_t(32) << 10;
+inline P2PPlan p2p_table_plan(const b200_comm *c, size_t wire_bytes, int count, bool whole_aligned) {
+  P2PPlan p = p2p_plan(c, nullptr, wire_bytes);
+  p.bulk = p.bulk && whole_aligned && wire_bytes / size_t(count) >= kP2PTableBulkMinAvg;
+  return p;
+}
+
 // All-to-all grid: at most one CTA per SM keeps it co-resident even with the bulk roles'
 // shared-memory ring.  Both sides of a pair derive their rings from this cap, so
 // b200_comm_set_blocks must be identical on every rank.
@@ -226,6 +246,11 @@ inline size_t a2a_own_ctas(size_t own_bytes) { return (own_bytes + (size_t(64) <
 constexpr size_t kGetSegBytes = size_t(256) << 10;
 inline bool get_bulk(const void *src, const void *dst, size_t nbytes) {
   return is_aligned16(src) && is_aligned16(dst) && (nbytes & 15) == 0 && nbytes >= kGetSegBytes;
+}
+// b200_get_multi: one table takes the bulk kernel when every entry is aligned whole units on both
+// ends and the entries average at least one bulk segment, the single get's threshold.
+inline bool get_table_bulk(size_t total_bytes, int count, bool whole_aligned) {
+  return whole_aligned && total_bytes / size_t(count) >= kGetSegBytes;
 }
 
 }  // namespace b200

@@ -6,7 +6,10 @@ Implements ``TensorTransportManager`` (python/ray/experimental/rdt/tensor_transp
 ``__ray_send__`` / ``__ray_recv__`` halves (run on the ``_ray_system`` concurrency-group thread,
 rdt_manager.py:655-681) map to ``collective.send`` / ``collective.recv`` of a collective group
 that contains both actors -- here a B200 group, so the payload moves through the
-sender-push NVLink kernel.  Two differences from the NCCL transport:
+sender-push NVLink kernel.  Three differences from the NCCL transport:
+
+* the tensors of an object travel as ONE message (``b200_send_multi`` / ``b200_recv_multi``): one
+  launch per side per 256 tensors instead of one per tensor;
 
 * ``can_abort_transport()`` is True: the device-side waits poll an abort word, so a stuck
   transfer is cancelled instead of Ray having to kill both actors (tensor_transport_manager.py:
@@ -161,8 +164,8 @@ class B200TensorTransport(TensorTransportManager):
         assert isinstance(communicator_metadata, B200CommunicatorMetadata)
         tensors = target_buffers or [torch.empty(tuple(shape), dtype=dtype, device="cuda")
                                      for shape, dtype in tensor_transport_metadata.tensor_meta]
-        for t in tensors:
-            _collective.recv(t, communicator_metadata.src_rank, communicator_metadata.communicator_name)
+        # the whole object is one message: one launch per table of tensors, not one per tensor
+        self._comm_of(communicator_metadata.communicator_name).recv_multi(tensors, communicator_metadata.src_rank)
         return tensors
 
     def send_multiple_tensors(self, tensors, tensor_transport_metadata, communicator_metadata) -> None:
@@ -171,7 +174,15 @@ class B200TensorTransport(TensorTransportManager):
         for t in tensors:
             if t.device.type != device.type:
                 raise ValueError(f"tensor device {t.device} does not match device {device}")
-            _collective.send(t, communicator_metadata.dst_rank, communicator_metadata.communicator_name)
+        self._comm_of(communicator_metadata.communicator_name).send_multi(tensors, communicator_metadata.dst_rank)
+
+    def _comm_of(self, group_name: str):
+        """The native endpoint (B200Comm) of a B200 collective group."""
+        group = _collective.get_group_handle(group_name)
+        comm = getattr(group, "comm", None)
+        if comm is None:
+            raise RuntimeError(f"collective group {group_name!r} is not a B200 group")
+        return comm
 
     def garbage_collect(self, obj_id, tensor_transport_meta, tensors) -> None:
         """Nothing is registered per object: the inbox ring is owned by the communicator."""
@@ -263,13 +274,6 @@ class B200IpcTransport(B200TensorTransport):
     def is_one_sided() -> bool:
         return True
 
-    def _comm_of(self, group_name: str):
-        group = _collective.get_group_handle(group_name)
-        comm = getattr(group, "comm", None)
-        if comm is None:
-            raise RuntimeError(f"collective group {group_name!r} is not a B200 group")
-        return comm
-
     def _arena(self, group_name: str, comm) -> "_HeapArena":
         if group_name not in self._arenas:
             _, size = comm.heap_range()
@@ -349,10 +353,10 @@ class B200IpcTransport(B200TensorTransport):
             stream.wait_event(local)  # same process (thread actors): IPC handles cannot be opened by their creator
         elif m.event_ipc_handle is not None:
             stream.wait_event(torch.cuda.Event.from_ipc_handle(device=device, handle=m.event_ipc_handle))
-        for t, off, nbytes in zip(tensors, m.heap_offsets, m.nbytes):
+        for t, nbytes in zip(tensors, m.nbytes):
             if t.numel() * t.element_size() != nbytes:
                 raise ValueError("target buffer size does not match the published tensor")
-            comm.get(t, m.src_rank, off)
+        comm.get_multi(tensors, m.src_rank, m.heap_offsets)  # the whole object in one launch
         return tensors
 
     def send_multiple_tensors(self, tensors, tensor_transport_metadata, communicator_metadata) -> None:

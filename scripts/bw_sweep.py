@@ -15,6 +15,9 @@ is bytes per peer: ``alltoall`` is the one-launch b200_alltoall, ``alltoall_p2p`
 it replaces (n-1 sends on the rank's stream, n-1 receives on a second stream, a local copy).
 --split skew gives them MoE-like splits instead: rank r sends size >> k bytes to rank r+k (4:2:1:...,
 the own segment the largest); --split local keeps `size` bytes on the rank and sends 16 KiB to each peer.
+``sendrecv_multi`` moves a tensor list from rank 0 to rank 1 in one launch per side
+(b200_send_multi / b200_recv_multi), ``sendrecv_loop`` with one send and one recv per tensor; the
+list comes from --tensors (N equal tensors of size / N bytes, or ResNet-50's parameter list).
 """
 import argparse
 import os
@@ -93,6 +96,27 @@ def alltoall_p2p(c, r, n, outs, ins, side):
     cur.wait_stream(side)
 
 
+def tensor_list_sizes(recipe, size):
+    """Byte sizes of the tensor list of a --tensors recipe: N equal tensors of size / N bytes, or the
+    fp32 parameters of torchvision's ResNet-50 (161 tensors, 102 MB; `size` is ignored)."""
+    if recipe == "resnet50":
+        import torchvision
+
+        return [p.numel() * 4 for p in torchvision.models.resnet50(weights=None).parameters()]
+    k = int(recipe)
+    return [max(size // k, 1)] * k
+
+
+def sendrecv_loop(c, r, sends, recvs):
+    """The per-tensor composition the one-launch list send / receive replaces."""
+    if r == 0:
+        for t in sends:
+            c.send(t, 1)
+    elif r == 1:
+        for t in recvs:
+            c.recv(t, 0)
+
+
 def grad_rs_unfused(c, out, grad, wout, scale, wire):
     """The composition the fused gradient reduce-scatter replaces: scale, cast to the wire type,
     reduce-scatter in the wire type, cast the shard back into the fp32 output."""
@@ -116,6 +140,9 @@ def main():
     ap.add_argument("--split", default="uniform", choices=["uniform", "skew", "local"],
                     help="all-to-all ops: bytes per peer (see above)")
     ap.add_argument("--wire", default="bfloat16", help="wire dtype of the grad_rs ops")
+    ap.add_argument("--tensors", default="1",
+                    help="sendrecv_multi / sendrecv_loop: comma list of recipes, N (N equal tensors of "
+                         "size / N bytes) or resnet50 (its fp32 parameter list, timed once)")
     args = ap.parse_args()
     n = args.world
     dtype = getattr(torch, args.dtype)
@@ -146,6 +173,8 @@ def main():
                 if algo == N.ALGO_LL and size > (64 << 10):
                     continue
                 for op in args.op.split(","):
+                    if op in ("sendrecv_multi", "sendrecv_loop"):
+                        continue  # timed per recipe below
                     if args.symm:
                         for c in g.comms:
                             c.symm_reset()
@@ -207,6 +236,25 @@ def main():
                     print(f"{op} {size:>11d} B  algo={aname:8s} blocks={blocks:3d} nvls_ctas={nctas:3d} {us:10.2f} us  "
                           f"algbw={algbw:8.1f} GB/s  busbw={algbw * factor:8.1f} GB/s", flush=True)
                     del xs
+        # tensor-list send / receive, rank 0 -> rank 1: the two ops alternate per (size, recipe)
+        list_ops = [op for op in args.op.split(",") if op in ("sendrecv_multi", "sendrecv_loop")]
+        for recipe in args.tensors.split(",") if list_ops else []:
+            if recipe == "resnet50" and size != args.min:
+                continue
+            sizes = tensor_list_sizes(recipe, size)
+            sends = [torch.ones(s, dtype=torch.uint8, device=g.device(0)) for s in sizes]
+            recvs = [torch.empty(s, dtype=torch.uint8, device=g.device(1)) for s in sizes]
+            for op in list_ops:
+                if op == "sendrecv_multi":
+                    call = lambda c, r: (c.send_multi(sends, 1) if r == 0 else  # noqa: E731
+                                         (c.recv_multi(recvs, 0) if r == 1 else None))
+                else:
+                    call = lambda c, r: sendrecv_loop(c, r, sends, recvs)  # noqa: E731
+                torch.cuda.synchronize()
+                us = time_graphs(g, call, iters)
+                total = sum(sizes)
+                print(f"{op} {total:>11d} B  tensors={recipe}({len(sizes)}) {us:10.2f} us  "
+                      f"algbw={total / us / 1e3:8.1f} GB/s", flush=True)
         size *= args.step
     g.destroy()
 
