@@ -235,6 +235,21 @@ int b200_recv_multi(b200_comm_t comm, void *const *bufs, const size_t *nbytes, i
 int b200_get_multi(b200_comm_t comm, void *const *dsts, int src_rank, const size_t *src_heap_offsets,
                    const size_t *nbytes, int ntensors, void *stream);
 
+/* In-place broadcast of a tensor LIST from root: bufs[i] (nbytes[i] bytes) on every rank receives
+ * root's bufs[i].  Sizes are in BYTES, so one list may mix dtypes; every rank passes the same size
+ * sequence.  A zero-size entry moves nothing and its pointer may be NULL.  Layout: the packed
+ * stream of b200_send_multi, tables of at most B200_P2P_TABLE_MAX non-empty entries in list order.
+ * Launches: one per window of at most staging_bytes of each table's stream, i.e. the sum over
+ * tables of ceil(16 * units / staging_bytes); a tensor may span windows.  Each launch runs
+ * b200_broadcast's protocol on the same staging slots and launch counter, so it interleaves with
+ * every other collective in stream order.  Refused calls (root out of range, ntensors < 0, NULL
+ * arrays with ntensors > 0, a NULL pointer with a non-zero size) launch nothing and return
+ * B200_ERR_INVALID; at world size 1, or when every entry is empty, nothing is launched.  Replaces
+ * c10d's flatten + ncclBroadcast + per-tensor copy-out of DDP's buffer sync
+ * (_broadcast_coalesced) and a loop of ncclBroadcast per tensor (weight sync). */
+int b200_broadcast_multi(b200_comm_t comm, void *const *bufs, const size_t *nbytes, int ntensors,
+                         int root, void *stream);
+
 /* Fused data-parallel gradient synchronisation (SURVEY K8): for a flat fp32
  * bucket computes grad[i] = sum_r wire(grad_r[i] * scale) in one launch, where
  * wire() is a cast to `wire_dtype` (B200_BF16 / B200_F16 compress the NVLink

@@ -9,6 +9,7 @@ from .collective import (
     allreduce,
     barrier,
     broadcast,
+    broadcast_multi,
     create_collective_group,
     destroy_collective_group,
     get_collective_group_size,
@@ -34,6 +35,6 @@ __all__ = [
     "B200Group", "BaseGroup", "Backend", "ReduceOp", "GroupManager", "types",
     "register_collective_backend", "init_collective_group", "create_collective_group",
     "destroy_collective_group", "is_group_initialized", "get_rank", "get_collective_group_size",
-    "get_group_handle", "allreduce", "barrier", "reduce", "broadcast", "allgather", "reducescatter",
+    "get_group_handle", "allreduce", "barrier", "reduce", "broadcast", "broadcast_multi", "allgather", "reducescatter",
     "send", "recv", "synchronize", "set_member_id", "use_manager",
 ]

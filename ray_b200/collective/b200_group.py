@@ -144,6 +144,16 @@ class B200Group(BaseGroup):
         root = len(tensors) * broadcast_options.root_rank + broadcast_options.root_tensor
         self._live().broadcast(t, root)
 
+    def broadcast_multi(self, tensors, src_rank: int = 0):
+        """Extension beyond the reference API (weight sync): broadcast a whole list of tensors, any
+        dtypes, from ``src_rank`` in place -- one launch per staging slot of packed data instead of
+        one ``broadcast`` per tensor.  Every rank passes tensors of the same byte sizes in order."""
+        if not isinstance(tensors, list):
+            raise RuntimeError("The input must be a list of tensors. Got '{}'.".format(type(tensors)))
+        if src_rank < 0 or src_rank >= self._world_size:
+            raise ValueError("rank '{}' is out of range for world size '{}'".format(src_rank, self._world_size))
+        self._live().broadcast_multi([_as_cuda_tensor(t) for t in tensors], src_rank)
+
     def allgather(self, tensor_lists, tensors, allgather_options=types.AllGatherOptions()):
         t = _unwrap_one(tensors)
         if not isinstance(tensor_lists, list) or len(tensor_lists) != 1:

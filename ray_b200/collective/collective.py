@@ -249,6 +249,20 @@ def broadcast(tensor, src_rank: int = 0, group_name: str = "default") -> None:
     g.broadcast([tensor], opts)
 
 
+def broadcast_multi(tensors: list, src_rank: int = 0, group_name: str = "default") -> None:
+    """Broadcast a list of tensors (any dtypes) from ``src_rank`` in place, as one call: an
+    extension beyond ``ray.util.collective`` for weight sync, where a loop of ``broadcast`` pays one
+    launch per parameter.  Every rank passes tensors of the same byte sizes in the same order; the
+    group's backend must provide ``broadcast_multi`` (``B200Group`` does)."""
+    _check_tensor_list_input(tensors)
+    g = get_group_handle(group_name)
+    _check_rank_valid(g, src_rank)
+    if not hasattr(g, "broadcast_multi"):
+        raise RuntimeError("The collective group '{}' ({}) has no list broadcast.".format(
+            group_name, type(g).__name__))
+    g.broadcast_multi(tensors, src_rank)
+
+
 def allgather(tensor_list: list, tensor, group_name: str = "default") -> None:
     _check_single_tensor_input(tensor)
     _check_tensor_list_input(tensor_list)

@@ -298,6 +298,17 @@ class B200Comm:
         N.check(self._lib.b200_broadcast(self._h, tensor.data_ptr(), tensor.numel(),
                                          dtype_code(tensor.dtype), int(root), self._stream()))
 
+    def broadcast_multi(self, tensors: Sequence[torch.Tensor], root: int = 0,
+                        stream: Optional[torch.cuda.Stream] = None) -> None:
+        """In-place broadcast of a list of tensors (any dtypes) from ``root``: one launch per
+        staging slot of packed data (per ``N.P2P_TABLE_MAX`` non-empty tensors at most) instead of
+        one per tensor.  Every rank passes tensors of the same byte sizes in the same order."""
+        ptrs, sizes = _tensor_list(tensors)
+        if not tensors:
+            return
+        N.check(self._lib.b200_broadcast_multi(self._h, ptrs, sizes, len(tensors), int(root),
+                                               stream.cuda_stream if stream is not None else self._stream()))
+
     def reduce(self, tensor: torch.Tensor, root: int = 0, op: int = N.SUM) -> None:
         _check_cuda_contiguous(tensor)
         N.check(self._lib.b200_reduce(self._h, tensor.data_ptr(), tensor.numel(),

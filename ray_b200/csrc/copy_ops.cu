@@ -1,7 +1,8 @@
 // copy_ops.cu — all-gather (SURVEY K2 with the K6 un-flatten copies fused away),
-// broadcast (K4) and the flag-only barrier (K7).  These kernels move bytes; they do
-// not depend on the element type.
+// broadcast (K4) of one tensor or of a tensor list, and the flag-only barrier (K7).
+// These kernels move bytes; they do not depend on the element type.
 #include "policy.h"
+#include "tensor_table.cuh"
 
 namespace b200 {
 
@@ -98,6 +99,50 @@ __global__ void __launch_bounds__(kThreads, 1) broadcast_kernel(DevComm c, Bcast
   finish_launch(c);
 }
 
+// One window of a table's packed stream (tensor_table.cuh): units [u0, u0 + units), at most one
+// staging slot.  The table stays in parameter space (__grid_constant__), indexed in place.
+struct BcastTableArgs {
+  P2PTable t;
+  size_t u0;
+  size_t units;
+  size_t staging_bytes;
+  int root;
+};
+
+// broadcast_kernel's protocol for a window of a table (b200_broadcast_multi): unit u0 + u of the
+// stream goes through byte u * 16 of the staging slot.
+template <bool NVLS>
+__global__ void __launch_bounds__(kThreads, 1)
+    broadcast_table_kernel(DevComm c, const __grid_constant__ BcastTableArgs a) {
+  const uint32_t launch = c.st->launch_ctr;
+  const uint32_t ep = launch * 4u;
+  const int r = c.rank;
+  const size_t U = a.units;
+  const size_t off = staging_slot_offset(launch, a.staging_bytes);
+  const size_t stride = size_t(gridDim.x) * kThreads;
+  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
+
+  if (r == a.root) {
+    char *dst = (NVLS ? c.mc_data : c.data[r]) + off;
+    for (size_t u = first; u < U; u += stride) {
+      const uint4 v = table_load_unit(a.t, a.u0 + u);
+      if (NVLS) multimem_st(dst + (u << 4), v);
+      else st_vec(dst + (u << 4), v);
+    }
+  }
+
+  if (!cta_barrier_all(c, ep + 1)) {
+    finish_launch(c);
+    return;
+  }
+
+  if (r != a.root) {
+    const char *src = (NVLS ? c.data[r] : c.data[a.root]) + off;
+    for (size_t u = first; u < U; u += stride) table_store_unit(a.t, a.u0 + u, ld_peer(src + (u << 4)));
+  }
+  finish_launch(c);
+}
+
 __global__ void barrier_kernel(DevComm c) {
   const uint32_t ep = c.st->launch_ctr * 4u;
   cta_barrier_all(c, ep + 1);
@@ -172,6 +217,35 @@ extern "C" int b200_broadcast(b200_comm_t c, void *buf, size_t count, int dtype,
     else broadcast_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
     B200_LAUNCH_CHECK(c);
     return B200_OK;
+  });
+}
+
+extern "C" int b200_broadcast_multi(b200_comm_t c, void *const *bufs, const size_t *nbytes, int ntensors, int root,
+                                    void *stream_) {
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_rank(c, root, "root")) ||
+      (rc = check_list(ntensors, bufs && nbytes)) || (rc = check_list_ptrs(bufs, nbytes, ntensors)))
+    return rc;
+  if (ntensors == 0 || c->world == 1) return B200_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  // One launch per window of at most one staging slot of each table's packed stream: a pure
+  // function of the size list and staging_bytes, so every rank makes the same launches.
+  return for_each_table(nbytes, ntensors, [&](int lo, int hi) -> int {
+    BcastTableArgs a{};
+    fill_table(a.t, bufs, nbytes, lo, hi);
+    a.staging_bytes = c->staging_bytes;
+    a.root = root;
+    const size_t total_units = a.t.ustart[a.t.count];
+    return for_each_piece(total_units, c->staging_bytes / 16, [&](size_t done, size_t units) -> int {
+      a.u0 = done;
+      a.units = units;
+      int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+      if (broadcast_nvls(c, units * 16)) broadcast_table_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
+      else broadcast_table_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
+      B200_LAUNCH_CHECK(c);
+      return B200_OK;
+    });
   });
 }
 

@@ -32,6 +32,7 @@
 
 #include "bulk_copy.cuh"
 #include "policy.h"
+#include "tensor_table.cuh"
 
 namespace b200 {
 
@@ -51,45 +52,15 @@ __device__ __forceinline__ bool cta_wait_flag(const DevComm &c, const uint32_t *
 
 // ---------------------------------------------------------------------------
 // Where the bytes of a message live: one contiguous buffer (char *), or a table of tensors
-// (b200_send_multi / b200_recv_multi).  A table's tensors form ONE packed message: tensor i
-// occupies 16-byte units [ustart[i], ustart[i+1]) with ustart[i+1] = ustart[i] + ceil(nbytes[i] / 16),
-// so no unit mixes two tensors.  The padding of a tensor's last unit travels on the wire (zeros)
-// and is never stored.  Entries are non-empty: the host drops zero-size ones on both sides.
+// (b200_send_multi / b200_recv_multi) whose packed stream of 16-byte units (tensor_table.cuh) is
+// the message.
 // ---------------------------------------------------------------------------
-struct P2PTable {
-  int count;
-  char *ptr[kP2PTableMax];
-  unsigned long long nbytes[kP2PTableMax];
-  unsigned long long ustart[kP2PTableMax + 1];
-};
-
 struct P2PTableArgs {
   P2PTable t;
   size_t nbytes;  // bytes on the wire: 16 * ustart[count]
   size_t chunk;
   int peer;
 };
-
-// the entry that owns unit u of a table's packed message (ustart strictly increasing)
-__device__ __forceinline__ int table_entry(const unsigned long long *start, int count, size_t u) {
-  int lo = 0, hi = count - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (start[mid] <= u) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
-}
-
-// unit u (of the whole message) of a table, loaded / stored like a unit of a user tensor
-__device__ __forceinline__ uint4 table_load_unit(const P2PTable &t, size_t u) {
-  const int i = table_entry(t.ustart, t.count, u);
-  return load_user_unit(t.ptr[i], u - t.ustart[i], make_units(t.nbytes[i]), is_aligned16(t.ptr[i]));
-}
-__device__ __forceinline__ void table_store_unit(const P2PTable &t, size_t u, uint4 v) {
-  const int i = table_entry(t.ustart, t.count, u);
-  store_user_unit(t.ptr[i], u - t.ustart[i], make_units(t.nbytes[i]), is_aligned16(t.ptr[i]), v);
-}
 
 // unit u of the chunk that starts at byte lo of the message
 __device__ __forceinline__ uint4 msg_load_unit(char *buf, size_t lo, size_t u, const Units &un, bool al) {
@@ -589,46 +560,6 @@ static int p2p_common(b200_comm *c, void *buf, size_t nbytes, int peer, cudaStre
 
 // ---- tensor lists -----------------------------------------------------------------------------
 
-// ntensors and the host arrays of a list entry point
-static int check_list(int ntensors, bool arrays) {
-  if (ntensors < 0) {
-    set_error("ntensors %d is negative", ntensors);
-    return B200_ERR_INVALID;
-  }
-  if (ntensors > 0 && !arrays) {
-    set_error("null argument array");
-    return B200_ERR_INVALID;
-  }
-  return B200_OK;
-}
-
-static int check_list_ptrs(const void *const *ptrs, const size_t *nbytes, int ntensors) {
-  for (int i = 0; i < ntensors; ++i) {
-    if (nbytes[i] && !ptrs[i]) {
-      set_error("tensor %d is null but has %zu bytes", i, nbytes[i]);
-      return B200_ERR_INVALID;
-    }
-  }
-  return B200_OK;
-}
-
-// Runs launch(lo, hi) over [0, ntensors) cut into runs of at most kP2PTableMax non-empty entries, in
-// list order.  The cut depends on the size list alone, so sender and receiver cut alike.
-template <typename Fn>
-static int for_each_table(const size_t *nbytes, int ntensors, Fn launch) {
-  int lo = 0, count = 0;
-  for (int i = 0; i < ntensors; ++i) {
-    if (!nbytes[i]) continue;
-    if (count == kP2PTableMax) {
-      if (int rc = launch(lo, i)) return rc;
-      lo = i;
-      count = 0;
-    }
-    ++count;
-  }
-  return count ? launch(lo, ntensors) : B200_OK;
-}
-
 static int p2p_multi_common(b200_comm *c, void *const *bufs, const size_t *nbytes, int ntensors, int peer,
                             cudaStream_t stream, bool send) {
   int rc;
@@ -642,15 +573,7 @@ static int p2p_multi_common(b200_comm *c, void *const *bufs, const size_t *nbyte
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   return for_each_table(nbytes, ntensors, [&](int lo, int hi) -> int {
     P2PTableArgs a{};
-    bool whole_aligned = true;
-    for (int i = lo; i < hi; ++i) {
-      if (!nbytes[i]) continue;
-      const int k = a.t.count++;
-      a.t.ptr[k] = static_cast<char *>(bufs[i]);
-      a.t.nbytes[k] = nbytes[i];
-      a.t.ustart[k + 1] = a.t.ustart[k] + (nbytes[i] + 15) / 16;
-      whole_aligned = whole_aligned && is_aligned16(bufs[i]) && (nbytes[i] & 15) == 0;
-    }
+    const bool whole_aligned = fill_table(a.t, bufs, nbytes, lo, hi);
     a.nbytes = size_t(a.t.ustart[a.t.count]) * 16;
     const P2PPlan p = p2p_table_plan(c, a.nbytes, a.t.count, whole_aligned);
     a.chunk = p.chunk;

@@ -2,8 +2,9 @@
 from .process_group import BACKEND_NAME, B200ProcessGroup, B200Work, register_b200_backend
 from .torch_config import (DEFAULT_GPU_BACKEND, B200TorchConfig, resolve_backend, setup_torch_process_group,
                            shutdown_torch, uses_b200)
-from .train_loop_utils import b200_fsdp_grad_hook, b200_grad_hook, get_device, prepare_model
+from .train_loop_utils import (B200DistributedDataParallel, b200_fsdp_grad_hook, b200_grad_hook, get_device,
+                               prepare_model)
 
 __all__ = ["BACKEND_NAME", "B200ProcessGroup", "B200Work", "register_b200_backend", "B200TorchConfig",
            "DEFAULT_GPU_BACKEND", "resolve_backend", "setup_torch_process_group", "shutdown_torch", "uses_b200",
-           "b200_grad_hook", "b200_fsdp_grad_hook", "get_device", "prepare_model"]
+           "B200DistributedDataParallel", "b200_grad_hook", "b200_fsdp_grad_hook", "get_device", "prepare_model"]

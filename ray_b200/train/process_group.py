@@ -255,6 +255,13 @@ class B200ProcessGroup(dist.ProcessGroup):
 
         return self._run(tensors, fn, tensors)
 
+    def broadcast_multi(self, tensors: List[torch.Tensor], root: int) -> B200Work:
+        """In-place broadcast of a list of contiguous CUDA tensors (any dtypes) from ``root`` in one
+        ``b200_broadcast_multi`` call: DDP's per-forward buffer sync without the flatten, the
+        per-dtype broadcasts and the per-tensor copy-out of c10d's ``_broadcast_coalesced``."""
+        return self._run(tensors, lambda comm: comm.broadcast_multi([self._contig(t) for t in tensors], root),
+                         tensors)
+
     def allgather(self, output_tensors, input_tensors, opts=None):
         if not self._all_cuda(input_tensors):
             return self._cpu_group().allgather(output_tensors, input_tensors, opts)

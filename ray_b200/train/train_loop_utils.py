@@ -9,6 +9,10 @@ when set, the DDP buckets are synchronised by ONE fused kernel per bucket (scale
 div + all-reduce (+ compress-hook casts).  Under ``parallel_strategy="fsdp"`` the same
 option reduce-scatters each FSDP unit's gradient with one fused kernel (scale, cast,
 reduce-scatter, cast back) instead of FSDP's div + fp32 reduce-scatter + div.
+
+Under ``"ddp"`` the wrapper is ``B200DistributedDataParallel``: on a b200 process group the buffer
+sync DDP runs before every forward (``broadcast_buffers=True``, the default) is one
+``b200_broadcast_multi`` call for all buffers of all dtypes.
 """
 from __future__ import annotations
 
@@ -91,6 +95,24 @@ def b200_fsdp_grad_hook(wire_dtype: torch.dtype = torch.bfloat16,
     return hook
 
 
+class B200DistributedDataParallel(DistributedDataParallel):
+    """``DistributedDataParallel`` whose per-forward buffer sync is one ``b200_broadcast_multi``
+    call on a b200 process group, instead of c10d's per-dtype flatten, broadcast and per-buffer
+    copy-out.  Everything else is DDP's, including the choice of the authoritative rank (which
+    ``Join`` moves off rank 0) and user-registered buffer hooks, which DDP calls instead of this
+    method."""
+
+    def _distributed_broadcast_coalesced(self, tensors, buffer_size, authoritative_rank=0):
+        pg = self.process_group
+        if isinstance(pg, B200ProcessGroup) and all(
+                t.is_cuda and t.is_contiguous() and t.device == self.device for t in tensors):
+            if tensors:
+                # stream-ordered: the caller's stream waits for the broadcast, the host does not
+                pg.broadcast_multi(list(tensors), authoritative_rank).wait()
+            return
+        super()._distributed_broadcast_coalesced(tensors, buffer_size, authoritative_rank)
+
+
 def prepare_model(model: torch.nn.Module, move_to_device: bool = True, parallel_strategy: Optional[str] = "ddp",
                   parallel_strategy_kwargs: Optional[Dict[str, Any]] = None,
                   gradient_wire_dtype: Optional[torch.dtype] = None) -> torch.nn.Module:
@@ -105,7 +127,7 @@ def prepare_model(model: torch.nn.Module, move_to_device: bool = True, parallel_
         if parallel_strategy == "ddp":
             if device.type != "cpu":
                 kwargs = {"device_ids": [device], "output_device": device, **kwargs}
-            model = DistributedDataParallel(model, **kwargs)
+            model = B200DistributedDataParallel(model, **kwargs)
             if gradient_wire_dtype is not None:
                 model.register_comm_hook(None, b200_grad_hook(gradient_wire_dtype))
         elif parallel_strategy == "fsdp":

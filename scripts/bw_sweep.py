@@ -3,7 +3,9 @@ GPU, launches replayed from CUDA graphs so host launch overhead does not pollute
 
     python scripts/bw_sweep.py --world 2 [--algos oneshot,twoshot,nvls] [--blocks 0,32,64] \
         [--min 1024 --max 1073741824] [--op allreduce|allgather|reducescatter|broadcast|sendrecv|grad|
-                                            grad_rs|grad_rs_unfused|alltoall|alltoall_p2p]
+                                            grad_rs|grad_rs_unfused|alltoall|alltoall_p2p|
+                                            sendrecv_multi|sendrecv_loop|bcast_multi|bcast_loop|
+                                            bcast_coalesced] [--tensors 16,256,resnet50,resnet50_buffers]
         [--split uniform|skew|local] [--wire bfloat16]
 
 Prints one line per (size, algo, blocks): us per launch, algbw, busbw (nccl-tests convention).
@@ -16,8 +18,12 @@ it replaces (n-1 sends on the rank's stream, n-1 receives on a second stream, a 
 --split skew gives them MoE-like splits instead: rank r sends size >> k bytes to rank r+k (4:2:1:...,
 the own segment the largest); --split local keeps `size` bytes on the rank and sends 16 KiB to each peer.
 ``sendrecv_multi`` moves a tensor list from rank 0 to rank 1 in one launch per side
-(b200_send_multi / b200_recv_multi), ``sendrecv_loop`` with one send and one recv per tensor; the
-list comes from --tensors (N equal tensors of size / N bytes, or ResNet-50's parameter list).
+(b200_send_multi / b200_recv_multi), ``sendrecv_loop`` with one send and one recv per tensor.
+``bcast_multi`` broadcasts a tensor list from rank 0 with b200_broadcast_multi, ``bcast_loop`` with
+one b200_broadcast per tensor, and ``bcast_coalesced`` the way DDP's buffer sync does through c10d
+today: flatten per dtype, one broadcast per dtype, a copy back into every tensor on the other ranks.
+The list comes from --tensors: N equal tensors of size / N bytes, ResNet-50's parameter list or
+ResNet-50's buffers (fp32 and int64).
 """
 import argparse
 import os
@@ -96,15 +102,20 @@ def alltoall_p2p(c, r, n, outs, ins, side):
     cur.wait_stream(side)
 
 
-def tensor_list_sizes(recipe, size):
-    """Byte sizes of the tensor list of a --tensors recipe: N equal tensors of size / N bytes, or the
-    fp32 parameters of torchvision's ResNet-50 (161 tensors, 102 MB; `size` is ignored)."""
-    if recipe == "resnet50":
+LIST_OPS = ("sendrecv_multi", "sendrecv_loop", "bcast_multi", "bcast_loop", "bcast_coalesced")
+
+
+def tensor_list_specs(recipe, size):
+    """(numel, dtype) of each tensor of a --tensors recipe: N equal uint8 tensors of size / N bytes,
+    the fp32 parameters of torchvision's ResNet-50 (161 tensors, 102 MB) or its buffers (159 tensors:
+    106 fp32, 53 int64, 208 KiB); `size` is ignored by the ResNet-50 recipes."""
+    if recipe in ("resnet50", "resnet50_buffers"):
         import torchvision
 
-        return [p.numel() * 4 for p in torchvision.models.resnet50(weights=None).parameters()]
+        m = torchvision.models.resnet50(weights=None)
+        return [(t.numel(), t.dtype) for t in (m.parameters() if recipe == "resnet50" else m.buffers())]
     k = int(recipe)
-    return [max(size // k, 1)] * k
+    return [(max(size // k, 1), torch.uint8)] * k
 
 
 def sendrecv_loop(c, r, sends, recvs):
@@ -115,6 +126,28 @@ def sendrecv_loop(c, r, sends, recvs):
     elif r == 1:
         for t in recvs:
             c.recv(t, 0)
+
+
+def bcast_loop(c, tensors):
+    """One b200_broadcast per tensor: what a weight sync over ray.util.collective.broadcast does."""
+    for t in tensors:
+        c.broadcast(t, 0)
+
+
+def bcast_coalesced(c, r, tensors):
+    """DDP's buffer sync through c10d's _broadcast_coalesced: one flat bucket per dtype, one
+    broadcast per bucket, a copy back into every tensor on the ranks other than the root.  With
+    c = None only the torch kernels run (to load them outside any collective)."""
+    by_dtype = {}
+    for t in tensors:
+        by_dtype.setdefault(t.dtype, []).append(t)
+    for ts in by_dtype.values():
+        flat = torch.cat([t.view(-1) for t in ts])
+        if c is not None:
+            c.broadcast(flat, 0)
+        if r != 0:
+            for t, f in zip(ts, flat.split([t.numel() for t in ts])):
+                t.view(-1).copy_(f)
 
 
 def grad_rs_unfused(c, out, grad, wout, scale, wire):
@@ -141,8 +174,9 @@ def main():
                     help="all-to-all ops: bytes per peer (see above)")
     ap.add_argument("--wire", default="bfloat16", help="wire dtype of the grad_rs ops")
     ap.add_argument("--tensors", default="1",
-                    help="sendrecv_multi / sendrecv_loop: comma list of recipes, N (N equal tensors of "
-                         "size / N bytes) or resnet50 (its fp32 parameter list, timed once)")
+                    help="list ops: comma list of recipes, N (N equal tensors of size / N bytes), "
+                         "resnet50 (its fp32 parameter list) or resnet50_buffers (its fp32 and int64 "
+                         "buffers); the resnet50 recipes are timed once")
     args = ap.parse_args()
     n = args.world
     dtype = getattr(torch, args.dtype)
@@ -173,7 +207,7 @@ def main():
                 if algo == N.ALGO_LL and size > (64 << 10):
                     continue
                 for op in args.op.split(","):
-                    if op in ("sendrecv_multi", "sendrecv_loop"):
+                    if op in LIST_OPS:
                         continue  # timed per recipe below
                     if args.symm:
                         for c in g.comms:
@@ -236,20 +270,32 @@ def main():
                     print(f"{op} {size:>11d} B  algo={aname:8s} blocks={blocks:3d} nvls_ctas={nctas:3d} {us:10.2f} us  "
                           f"algbw={algbw:8.1f} GB/s  busbw={algbw * factor:8.1f} GB/s", flush=True)
                     del xs
-        # tensor-list send / receive, rank 0 -> rank 1: the two ops alternate per (size, recipe)
-        list_ops = [op for op in args.op.split(",") if op in ("sendrecv_multi", "sendrecv_loop")]
+        # tensor lists: send / receive rank 0 -> rank 1, broadcast from rank 0; the ops alternate per
+        # (size, recipe)
+        list_ops = [op for op in args.op.split(",") if op in LIST_OPS]
         for recipe in args.tensors.split(",") if list_ops else []:
-            if recipe == "resnet50" and size != args.min:
+            if recipe.startswith("resnet50") and size != args.min:
                 continue
-            sizes = tensor_list_sizes(recipe, size)
+            specs = tensor_list_specs(recipe, size)
+            sizes = [k * torch.empty((), dtype=dt).element_size() for k, dt in specs]
             sends = [torch.ones(s, dtype=torch.uint8, device=g.device(0)) for s in sizes]
             recvs = [torch.empty(s, dtype=torch.uint8, device=g.device(1)) for s in sizes]
+            lists = [[torch.ones(k, dtype=dt, device=g.device(r)) for k, dt in specs] for r in range(n)]
+            for r in range(n):
+                with torch.cuda.device(g.devices[r]):
+                    bcast_coalesced(None, r, lists[r])
             for op in list_ops:
                 if op == "sendrecv_multi":
                     call = lambda c, r: (c.send_multi(sends, 1) if r == 0 else  # noqa: E731
                                          (c.recv_multi(recvs, 0) if r == 1 else None))
-                else:
+                elif op == "sendrecv_loop":
                     call = lambda c, r: sendrecv_loop(c, r, sends, recvs)  # noqa: E731
+                elif op == "bcast_multi":
+                    call = lambda c, r: c.broadcast_multi(lists[r], 0)  # noqa: E731
+                elif op == "bcast_loop":
+                    call = lambda c, r: bcast_loop(c, lists[r])  # noqa: E731
+                else:
+                    call = lambda c, r: bcast_coalesced(c, r, lists[r])  # noqa: E731
                 torch.cuda.synchronize()
                 us = time_graphs(g, call, iters)
                 total = sum(sizes)
