@@ -250,6 +250,41 @@ int b200_get_multi(b200_comm_t comm, void *const *dsts, int src_rank, const size
 int b200_broadcast_multi(b200_comm_t comm, void *const *bufs, const size_t *nbytes, int ntensors,
                          int root, void *stream);
 
+/* All-gather of a tensor LIST: outs has ntensors * world_size entries, and outs[i * world_size + p]
+ * (nbytes[i] bytes) receives rank p's ins[i].  Sizes are in BYTES, so one list may mix dtypes; every
+ * rank passes the same size sequence.  A zero-size entry moves nothing and its pointers may be NULL.
+ * The only overlap allowed is c10d's in-place form, outs[i * world_size + this rank] == ins[i]; no
+ * other output may overlap an input.  Layout: the packed stream of b200_send_multi over the inputs,
+ * tables of at most B200_P2P_TABLE_MAX non-empty entries in list order.  Launches: one per window of
+ * at most staging_bytes of each table's stream, i.e. the sum over tables of
+ * ceil(16 * units / staging_bytes), a function of the size list and staging_bytes alone.  Each launch
+ * runs b200_allgather's staged protocol on the same staging slots and launch counter, so it
+ * interleaves with every other collective in stream order.  Refused calls (ntensors < 0, NULL arrays
+ * with ntensors > 0, a NULL pointer with a non-zero size) launch nothing and return
+ * B200_ERR_INVALID.  At world size 1 every entry that is not in place is copied with
+ * cudaMemcpyAsync; a list that is empty, or whose entries are all empty, launches nothing.  Replaces
+ * one ncclAllGather per tensor of c10d's coalesced all-gather (allgather_into_tensor_coalesced,
+ * allgather_coalesced). */
+int b200_allgather_multi(b200_comm_t comm, const void *const *ins, const size_t *nbytes, int ntensors,
+                         void *const *outs, void *stream);
+
+/* Reduce-scatter of a tensor LIST: ins has ntensors * world_size entries, and ins[i * world_size + q]
+ * (counts[i] elements) is this rank's contribution to rank q's outs[i]; outs[i] = op over ranks of
+ * (that rank's ins[i * world_size + this rank]), reduced rank-ascending.  One dtype and one op per
+ * call; every rank passes the same count sequence.  The result is bit-identical to b200_reducescatter
+ * run on each tensor alone.  A zero-count entry moves nothing and its pointers may be NULL.  The only
+ * overlap allowed is c10d's in-place form, outs[i] == ins[i * world_size + this rank].  Launches:
+ * outputs are packed as in b200_allgather_multi, and each table's stream of output units is cut into
+ * windows of at most floor(staging_bytes / (16 * world_size)) units (the world_size sub-slots of a
+ * window fill one staging slot), one launch each, on the same staging slots and launch counter as
+ * every other collective.  Refused calls (ntensors < 0, NULL arrays with ntensors > 0, a NULL pointer
+ * with a non-zero count) launch nothing and return B200_ERR_INVALID; a bad dtype or op returns
+ * B200_ERR_UNSUPPORTED as in b200_reducescatter.  At world size 1 every entry that is not in place is
+ * copied with cudaMemcpyAsync (AVG over one rank is the identity).  Replaces one ncclReduceScatter
+ * per tensor of c10d's coalesced reduce-scatter (reduce_scatter_tensor_coalesced). */
+int b200_reducescatter_multi(b200_comm_t comm, const void *const *ins, void *const *outs,
+                             const size_t *counts, int ntensors, int dtype, int op, void *stream);
+
 /* Fused data-parallel gradient synchronisation (SURVEY K8): for a flat fp32
  * bucket computes grad[i] = sum_r wire(grad_r[i] * scale) in one launch, where
  * wire() is a cast to `wire_dtype` (B200_BF16 / B200_F16 compress the NVLink

@@ -14,7 +14,7 @@ LIB_NAME = "libb200_collective.so"
 LIB_PATH = Path(__file__).resolve().parent / LIB_NAME
 HANDLE_BYTES = 256
 MAX_RANKS = 8
-P2P_TABLE_MAX = 256  # B200_P2P_TABLE_MAX: non-empty tensors per table of the list send / recv / get / broadcast
+P2P_TABLE_MAX = 256  # B200_P2P_TABLE_MAX: non-empty tensors per table of every list call
 
 # status codes (b200_status_t)
 OK = 0
@@ -99,6 +99,10 @@ SIGNATURES = {
     "b200_get_multi": (c_int, [c_void_p, POINTER(c_void_p), c_int, POINTER(c_size_t), POINTER(c_size_t), c_int,
                                c_void_p]),
     "b200_broadcast_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, c_int, c_void_p]),
+    "b200_allgather_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(c_void_p),
+                                     c_void_p]),
+    "b200_reducescatter_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_size_t), c_int,
+                                         c_int, c_int, c_void_p]),
     "b200_grad_allreduce": (c_int, [c_void_p, c_void_p, c_size_t, c_float, c_int, c_void_p]),
     "b200_grad_reducescatter": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_float, c_int, c_void_p]),
     "b200_allreduce_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, c_int, c_int, c_void_p]),

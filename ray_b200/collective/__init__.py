@@ -6,6 +6,7 @@ from .base_group import BaseGroup
 from .collective import (
     GroupManager,
     allgather,
+    allgather_multi,
     allreduce,
     barrier,
     broadcast,
@@ -20,6 +21,7 @@ from .collective import (
     recv,
     reduce,
     reducescatter,
+    reducescatter_multi,
     send,
     set_member_id,
     synchronize,
@@ -35,6 +37,6 @@ __all__ = [
     "B200Group", "BaseGroup", "Backend", "ReduceOp", "GroupManager", "types",
     "register_collective_backend", "init_collective_group", "create_collective_group",
     "destroy_collective_group", "is_group_initialized", "get_rank", "get_collective_group_size",
-    "get_group_handle", "allreduce", "barrier", "reduce", "broadcast", "broadcast_multi", "allgather", "reducescatter",
-    "send", "recv", "synchronize", "set_member_id", "use_manager",
+    "get_group_handle", "allreduce", "barrier", "reduce", "broadcast", "broadcast_multi", "allgather", "allgather_multi",
+    "reducescatter", "reducescatter_multi", "send", "recv", "synchronize", "set_member_id", "use_manager",
 ]

@@ -174,6 +174,44 @@ class B200Group(BaseGroup):
         _check_same_shape_dtype(out, ins)
         self._live().reducescatter(out, ins, _op_code(reducescatter_options.reduceOp))
 
+    def allgather_multi(self, tensor_lists, tensors):
+        """Extension beyond the reference API: ``allgather`` of a whole list of tensors (any dtypes)
+        -- ``tensor_lists[i][p]`` receives rank p's ``tensors[i]`` -- in one launch per staging slot
+        of packed data instead of one per tensor.  Every rank passes the same sizes in order."""
+        if not isinstance(tensors, list) or not isinstance(tensor_lists, list):
+            raise RuntimeError("The inputs must be lists of tensors. Got '{}' and '{}'.".format(
+                type(tensor_lists), type(tensors)))
+        if len(tensor_lists) != len(tensors):
+            raise RuntimeError("expected one output tensor list per input tensor")
+        ins = [_as_cuda_tensor(t) for t in tensors]
+        out_lists = []
+        for lst, t in zip(tensor_lists, ins):
+            outs = [_as_cuda_tensor(o) for o in lst]
+            if len(outs) != self._world_size:
+                raise RuntimeError("The length of the tensor list operands to allgather must be equal to world_size.")
+            _check_same_shape_dtype(t, outs)
+            out_lists.append(outs)
+        self._live().allgather_multi(out_lists, ins)
+
+    def reducescatter_multi(self, tensors, tensor_lists, op=ReduceOp.SUM):
+        """Extension beyond the reference API: ``reducescatter`` of a whole list of tensors of one
+        dtype -- ``tensors[i]`` = op over ranks of that rank's ``tensor_lists[i][this rank]`` -- in
+        one launch per window of packed data, bit-identical to one ``reducescatter`` per tensor."""
+        if not isinstance(tensors, list) or not isinstance(tensor_lists, list):
+            raise RuntimeError("The inputs must be lists of tensors. Got '{}' and '{}'.".format(
+                type(tensors), type(tensor_lists)))
+        if len(tensor_lists) != len(tensors):
+            raise RuntimeError("expected one input tensor list per output tensor")
+        outs = [_as_cuda_tensor(t) for t in tensors]
+        in_lists = []
+        for out, lst in zip(outs, tensor_lists):
+            ins = [_as_cuda_tensor(i) for i in lst]
+            if len(ins) != self._world_size:
+                raise RuntimeError("The length of the tensor list operands to reducescatter must be equal to world_size.")
+            _check_same_shape_dtype(out, ins)
+            in_lists.append(ins)
+        self._live().reducescatter_multi(outs, in_lists, _op_code(op))
+
     def send(self, tensors, send_options=types.SendOptions()):
         t = _unwrap_one(tensors)
         self._check_peer(send_options.dst_rank)

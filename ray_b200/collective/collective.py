@@ -283,6 +283,47 @@ def reducescatter(tensor, tensor_list: list, group_name: str = "default", op=typ
     g.reducescatter([tensor], [tensor_list], opts)
 
 
+def _check_list_of_lists(tensor_lists, tensors, world_size: int, what: str) -> None:
+    if not isinstance(tensor_lists, list):
+        raise RuntimeError("The input must be a list of tensor lists. Got '{}'.".format(type(tensor_lists)))
+    if len(tensor_lists) != len(tensors):
+        raise RuntimeError("Got {} tensor lists for {} tensors.".format(len(tensor_lists), len(tensors)))
+    for lst in tensor_lists:
+        _check_tensor_list_input(lst)
+        if len(lst) != world_size:
+            raise RuntimeError(
+                "The length of the tensor list operands to {} must be equal to world_size.".format(what))
+
+
+def allgather_multi(tensor_lists: list, tensors: list, group_name: str = "default") -> None:
+    """``allgather`` of a list of tensors (any dtypes) as one call: ``tensor_lists[i][p]`` receives
+    rank p's ``tensors[i]``.  An extension beyond ``ray.util.collective`` for sharded parameters,
+    where a loop of ``allgather`` pays one launch per tensor.  Every rank passes tensors of the same
+    byte sizes in the same order; the group's backend must provide ``allgather_multi``
+    (``B200Group`` does)."""
+    _check_tensor_list_input(tensors)
+    g = get_group_handle(group_name)
+    _check_list_of_lists(tensor_lists, tensors, g.world_size, "allgather")
+    if not hasattr(g, "allgather_multi"):
+        raise RuntimeError("The collective group '{}' ({}) has no list all-gather.".format(
+            group_name, type(g).__name__))
+    g.allgather_multi(tensor_lists, tensors)
+
+
+def reducescatter_multi(tensors: list, tensor_lists: list, group_name: str = "default",
+                        op=types.ReduceOp.SUM) -> None:
+    """``reducescatter`` of a list of tensors of one dtype as one call: ``tensors[i]`` = op over ranks
+    of that rank's ``tensor_lists[i][this rank]``.  The mirror image of ``allgather_multi``; the
+    group's backend must provide ``reducescatter_multi`` (``B200Group`` does)."""
+    _check_tensor_list_input(tensors)
+    g = get_group_handle(group_name)
+    _check_list_of_lists(tensor_lists, tensors, g.world_size, "reducescatter")
+    if not hasattr(g, "reducescatter_multi"):
+        raise RuntimeError("The collective group '{}' ({}) has no list reduce-scatter.".format(
+            group_name, type(g).__name__))
+    g.reducescatter_multi(tensors, tensor_lists, op)
+
+
 def send(tensor, dst_rank: int, group_name: str = "default") -> None:
     _check_single_tensor_input(tensor)
     g = get_group_handle(group_name)

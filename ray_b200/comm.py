@@ -293,6 +293,103 @@ class B200Comm:
         N.check(self._lib.b200_reducescatter(self._h, arr, out.data_ptr(), out.numel(),
                                              dtype_code(out.dtype), int(op), self._stream()))
 
+    def allgather_multi(self, out_lists: Sequence[Sequence[torch.Tensor]], tensors: Sequence[torch.Tensor]) -> None:
+        """``allgather`` of a list of tensors (any dtypes): ``out_lists[i][p]`` receives rank p's
+        ``tensors[i]``.  One launch per staging slot of packed data (per ``N.P2P_TABLE_MAX``
+        non-empty tensors at most) instead of one per tensor.  Every rank passes tensors of the same
+        byte sizes in the same order; ``out_lists[i][this rank]`` may be ``tensors[i]`` itself."""
+        n = self.world_size
+        if len(out_lists) != len(tensors):
+            raise RuntimeError(f"allgather_multi got {len(out_lists)} output lists for {len(tensors)} tensors")
+        ptrs, sizes = _tensor_list(tensors)
+        outs = (ctypes.c_void_p * max(len(tensors) * n, 1))()
+        for i, (lst, t) in enumerate(zip(out_lists, tensors)):
+            if len(lst) != n:
+                raise RuntimeError("The length of the tensor list operands to allgather must be equal to world_size.")
+            for p, o in enumerate(lst):
+                _check_cuda_contiguous(o, "output tensor")
+                if o.dtype != t.dtype or o.numel() != t.numel():
+                    raise RuntimeError("All tensor operands to allgather must have the same dtype and size.")
+                outs[i * n + p] = o.data_ptr()
+        if not tensors:
+            return
+        N.check(self._lib.b200_allgather_multi(self._h, ptrs, sizes, len(tensors), outs, self._stream()))
+
+    def allgather_into_multi(self, outs: Sequence[torch.Tensor], tensors: Sequence[torch.Tensor]) -> None:
+        """``allgather_into`` of a list of tensors (any dtypes) in one ``b200_allgather_multi`` call:
+        ``outs[i]`` is the rank-major concatenation of every rank's ``tensors[i]`` (the
+        ``all_gather_into_tensor`` layout)."""
+        n = self.world_size
+        if len(outs) != len(tensors):
+            raise RuntimeError(f"allgather_into_multi got {len(outs)} outputs for {len(tensors)} tensors")
+        ptrs, sizes = _tensor_list(tensors)
+        arr = (ctypes.c_void_p * max(len(tensors) * n, 1))()
+        for i, (o, t) in enumerate(zip(outs, tensors)):
+            _check_cuda_contiguous(o, "output tensor")
+            if o.dtype != t.dtype or o.numel() != t.numel() * n:
+                raise RuntimeError("allgather output must hold world_size copies of the input")
+            for p in range(n):
+                arr[i * n + p] = o.data_ptr() + p * sizes[i]
+        if not tensors:
+            return
+        N.check(self._lib.b200_allgather_multi(self._h, ptrs, sizes, len(tensors), arr, self._stream()))
+
+    def _reducescatter_multi(self, outs: Sequence[torch.Tensor], ins, op: int) -> None:
+        """outs[i] = reduce over ranks of (that rank's ins[i * world_size + this rank]); ``ins`` is a
+        flat pointer array."""
+        ptrs = (ctypes.c_void_p * max(len(outs), 1))()
+        counts = (ctypes.c_size_t * max(len(outs), 1))()
+        for i, o in enumerate(outs):
+            ptrs[i] = o.data_ptr()
+            counts[i] = o.numel()
+        if not outs:
+            return
+        N.check(self._lib.b200_reducescatter_multi(self._h, ins, ptrs, counts, len(outs), dtype_code(outs[0].dtype),
+                                                   int(op), self._stream()))
+
+    def _check_rs_outputs(self, outs: Sequence[torch.Tensor], n_in: int) -> None:
+        if len(outs) != n_in:
+            raise RuntimeError(f"reducescatter list got {len(outs)} outputs for {n_in} inputs")
+        for i, o in enumerate(outs):
+            _check_cuda_contiguous(o, f"output tensor {i}")
+            if o.dtype != outs[0].dtype:
+                raise RuntimeError("All tensor operands to a list reducescatter must have the same dtype.")
+
+    def reducescatter_multi(self, outs: Sequence[torch.Tensor], in_lists: Sequence[Sequence[torch.Tensor]],
+                            op: int = N.SUM) -> None:
+        """``reducescatter`` of a list of tensors of one dtype: ``outs[i]`` = op over ranks of that
+        rank's ``in_lists[i][this rank]``, bit-identical to one ``reducescatter`` per tensor, in one
+        launch per window of packed data.  ``outs[i]`` may be ``in_lists[i][this rank]`` itself."""
+        n = self.world_size
+        self._check_rs_outputs(outs, len(in_lists))
+        arr = (ctypes.c_void_p * max(len(outs) * n, 1))()
+        for i, (o, lst) in enumerate(zip(outs, in_lists)):
+            if len(lst) != n:
+                raise RuntimeError("The length of the tensor list operands to reducescatter must be equal to world_size.")
+            for q, t in enumerate(lst):
+                _check_cuda_contiguous(t)
+                if t.dtype != o.dtype or t.numel() != o.numel():
+                    raise RuntimeError("All tensor operands to reducescatter must have the same dtype and size.")
+                arr[i * n + q] = t.data_ptr()
+        self._reducescatter_multi(outs, arr, op)
+
+    def reducescatter_from_multi(self, outs: Sequence[torch.Tensor], tensors: Sequence[torch.Tensor],
+                                 op: int = N.SUM) -> None:
+        """``reducescatter_from`` of a list of tensors of one dtype in one ``b200_reducescatter_multi``
+        call: ``outs[i]`` = op over ranks of this rank's 1/world slice of ``tensors[i]`` (the
+        ``reduce_scatter_tensor`` layout)."""
+        n = self.world_size
+        self._check_rs_outputs(outs, len(tensors))
+        arr = (ctypes.c_void_p * max(len(outs) * n, 1))()
+        for i, (o, t) in enumerate(zip(outs, tensors)):
+            _check_cuda_contiguous(t, f"tensor {i}")
+            if t.dtype != o.dtype or o.numel() * n != t.numel():
+                raise RuntimeError("reducescatter input must hold world_size slices of the output size")
+            step = o.numel() * o.element_size()
+            for q in range(n):
+                arr[i * n + q] = t.data_ptr() + q * step
+        self._reducescatter_multi(outs, arr, op)
+
     def broadcast(self, tensor: torch.Tensor, root: int = 0) -> None:
         _check_cuda_contiguous(tensor)
         N.check(self._lib.b200_broadcast(self._h, tensor.data_ptr(), tensor.numel(),

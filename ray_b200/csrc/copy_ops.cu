@@ -1,5 +1,5 @@
-// copy_ops.cu — all-gather (SURVEY K2 with the K6 un-flatten copies fused away),
-// broadcast (K4) of one tensor or of a tensor list, and the flag-only barrier (K7).
+// copy_ops.cu — all-gather (SURVEY K2 with the K6 un-flatten copies fused away) and
+// broadcast (K4), each of one tensor or of a tensor list, and the flag-only barrier (K7).
 // These kernels move bytes; they do not depend on the element type.
 #include "policy.h"
 #include "tensor_table.cuh"
@@ -143,6 +143,62 @@ __global__ void __launch_bounds__(kThreads, 1)
   finish_launch(c);
 }
 
+// One window [u0, u0 + units) of a table's packed stream of input units, at most one staging slot.
+struct AGTableArgs {
+  P2PTable t;                           // the inputs
+  char *outs[kP2PTableMax][kMaxRanks];  // outs[k][p]: packed entry k's output for rank p
+  size_t u0;
+  size_t units;
+  size_t staging_bytes;
+};
+static_assert(fits_param_space<AGTableArgs>(), "all-gather table exceeds the kernel parameter space");
+
+// allgather_kernel's protocol for a window of a table (b200_allgather_multi): every rank stages
+// unit u0 + u of its stream at byte u * 16 of its own slot, then pulls each peer's slot into
+// the owning entry's output for that peer.
+__global__ void __launch_bounds__(kThreads, 1)
+    allgather_table_kernel(DevComm c, const __grid_constant__ AGTableArgs a) {
+  const uint32_t launch = c.st->launch_ctr;
+  const uint32_t ep = launch * 4u;
+  const int n = c.world, r = c.rank;
+  const size_t U = a.units;
+  const size_t off = staging_slot_offset(launch, a.staging_bytes);
+  const size_t stride = size_t(gridDim.x) * kThreads;
+  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
+
+  char *mine = c.data[r] + off;
+  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), table_load_unit(a.t, a.u0 + u));
+
+  if (!cta_barrier_all(c, ep + 1)) {
+    finish_launch(c);
+    return;
+  }
+
+  for (size_t u = first; u < U; u += stride) {
+    const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
+    const size_t lu = a.u0 + u - a.t.ustart[k];
+    const Units un = make_units(a.t.nbytes[k]);
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int p = r + i;
+        if (p >= n) p -= n;
+        v[i] = ld_peer(c.data[p] + off + (u << 4));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int p = r + i;
+        if (p >= n) p -= n;
+        store_user_unit(a.outs[k][p], lu, un, is_aligned16(a.outs[k][p]), v[i]);
+      }
+    }
+  }
+  finish_launch(c);
+}
+
 __global__ void barrier_kernel(DevComm c) {
   const uint32_t ep = c.st->launch_ctr * 4u;
   cta_barrier_all(c, ep + 1);
@@ -229,24 +285,56 @@ extern "C" int b200_broadcast_multi(b200_comm_t c, void *const *bufs, const size
   if (ntensors == 0 || c->world == 1) return B200_OK;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
-  // One launch per window of at most one staging slot of each table's packed stream: a pure
-  // function of the size list and staging_bytes, so every rank makes the same launches.
-  return for_each_table(nbytes, ntensors, [&](int lo, int hi) -> int {
-    BcastTableArgs a{};
-    fill_table(a.t, bufs, nbytes, lo, hi);
-    a.staging_bytes = c->staging_bytes;
-    a.root = root;
-    const size_t total_units = a.t.ustart[a.t.count];
-    return for_each_piece(total_units, c->staging_bytes / 16, [&](size_t done, size_t units) -> int {
-      a.u0 = done;
-      a.units = units;
-      int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
-      if (broadcast_nvls(c, units * 16)) broadcast_table_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
-      else broadcast_table_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
-      B200_LAUNCH_CHECK(c);
-      return B200_OK;
-    });
-  });
+  // One launch per window of at most one staging slot of each table's packed stream.
+  BcastTableArgs a{};
+  a.staging_bytes = c->staging_bytes;
+  a.root = root;
+  return for_each_window(a.t, bufs, nbytes, ntensors, c->staging_bytes / 16, [](int, int) {},
+                         [&](size_t done, size_t units) -> int {
+                           a.u0 = done;
+                           a.units = units;
+                           int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+                           if (broadcast_nvls(c, units * 16))
+                             broadcast_table_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
+                           else broadcast_table_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
+                           B200_LAUNCH_CHECK(c);
+                           return B200_OK;
+                         });
+}
+
+extern "C" int b200_allgather_multi(b200_comm_t c, const void *const *ins, const size_t *nbytes, int ntensors,
+                                    void *const *outs, void *stream_) {
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_list(ntensors, ins && nbytes && outs)) ||
+      (rc = check_list_ptrs(ins, nbytes, ntensors)) ||
+      (rc = check_list_rank_ptrs(outs, nbytes, ntensors, c->world, "output")))
+    return rc;
+  if (ntensors == 0) return B200_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  const int n = c->world;
+  if (n == 1) {
+    for (int i = 0; i < ntensors; ++i)
+      if (nbytes[i] && outs[i] != ins[i])
+        B200_CHECK_CUDA(cudaMemcpyAsync(outs[i], ins[i], nbytes[i], cudaMemcpyDeviceToDevice, stream));
+    return B200_OK;
+  }
+  // One launch per window of at most one staging slot of each table's stream of input units.
+  AGTableArgs a{};
+  a.staging_bytes = c->staging_bytes;
+  return for_each_window(
+      a.t, const_cast<void *const *>(ins), nbytes, ntensors, c->staging_bytes / 16,
+      [&](int k, int i) {
+        for (int p = 0; p < n; ++p) a.outs[k][p] = static_cast<char *>(outs[size_t(i) * n + p]);
+      },
+      [&](size_t done, size_t units) -> int {
+        a.u0 = done;
+        a.units = units;
+        int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+        allgather_table_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
+        B200_LAUNCH_CHECK(c);
+        return B200_OK;
+      });
 }
 
 extern "C" int b200_barrier(b200_comm_t c, void *stream_) {

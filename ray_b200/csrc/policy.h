@@ -207,8 +207,9 @@ inline P2PPlan p2p_plan(const b200_comm *c, const void *buf, size_t nbytes) {
 // Tensor lists (b200_send_multi / b200_recv_multi / b200_get_multi) travel as tables of at most
 // kP2PTableMax non-empty entries, one launch per table.  The table is a __grid_constant__ kernel
 // parameter: CUDA >= 12.1 allows 32764 bytes of parameters on sm_90, and 256 entries take about
-// 6 KiB (send / recv) or 8 KiB (get).  What a parameter block that large costs per launch has not
-// been measured.
+// 6 KiB (send / recv / broadcast), 8 KiB (get) or 22 KiB (all-gather / reduce-scatter, which add
+// kMaxRanks per-rank pointers to each entry).  What a parameter block that large costs per launch
+// has not been measured in isolation.
 constexpr int kP2PTableMax = B200_P2P_TABLE_MAX;
 
 // A table is ONE message of 16 * (sum of ceil(nbytes[i] / 16)) bytes: the protocol (chunk, rings)

@@ -5,8 +5,12 @@
 // caller's list and writes tensor q into sub-slot r of rank q's staging slot over
 // NVLink (the local copy-in and the transfer are the same instruction stream).  After
 // one barrier every rank reduces its n sub-slots from local HBM, rank-ascending, into
-// the caller's output tensor.
+// the caller's output tensor.  The list form (b200_reducescatter_multi) runs the same protocol
+// over windows of a packed tensor table (tensor_table.cuh).
+#include <vector>
+
 #include "policy.h"
+#include "tensor_table.cuh"
 
 namespace b200 {
 
@@ -63,6 +67,70 @@ __global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, R
     for (int p = 0; p < kMaxRanks; ++p)
       if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
     store_user_unit(a.out, u, un, out_al, reduce_ranks<T, OP>(v, n));
+  }
+  finish_launch(c);
+}
+
+// One window [u0, u0 + units) of a table's packed stream of output units; n sub-slots of
+// units * 16 bytes fit one staging slot.
+struct RSTableArgs {
+  P2PTable t;                                // the outputs
+  const char *ins[kP2PTableMax][kMaxRanks];  // ins[k][q]: packed entry k's contribution to rank q
+  size_t u0;
+  size_t units;
+  size_t staging_bytes;
+};
+static_assert(fits_param_space<RSTableArgs>(), "reduce-scatter table exceeds the kernel parameter space");
+
+// reducescatter_kernel's push protocol for a window of a table (b200_reducescatter_multi): unit
+// u0 + u of entry k's input for rank q goes to byte r * units * 16 + u * 16 of rank q's slot.
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1)
+    reducescatter_table_kernel(DevComm c, const __grid_constant__ RSTableArgs a) {
+  const uint32_t launch = c.st->launch_ctr;
+  const uint32_t ep = launch * 4u;
+  const int n = c.world, r = c.rank;
+  const size_t U = a.units;
+  const size_t sub = U << 4;  // bytes per sub-slot
+  const size_t off = staging_slot_offset(launch, a.staging_bytes);
+  const size_t stride = size_t(gridDim.x) * kThreads;
+  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
+
+  for (size_t u = first; u < U; u += stride) {
+    const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
+    const size_t lu = a.u0 + u - a.t.ustart[k];
+    const Units un = make_units(a.t.nbytes[k]);
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int q = r + i;
+        if (q >= n) q -= n;
+        v[i] = load_user_unit(a.ins[k][q], lu, un, is_aligned16(a.ins[k][q]));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int q = r + i;
+        if (q >= n) q -= n;
+        st_vec(c.data[q] + off + size_t(r) * sub + (u << 4), v[i]);
+      }
+    }
+  }
+
+  if (!cta_barrier_all(c, ep + 1)) {
+    finish_launch(c);
+    return;
+  }
+
+  const char *mine = c.data[r] + off;
+  for (size_t u = first; u < U; u += stride) {
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int p = 0; p < kMaxRanks; ++p)
+      if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
+    table_store_unit(a.t, a.u0 + u, reduce_ranks<T, OP>(v, n));
   }
   finish_launch(c);
 }
@@ -163,6 +231,49 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
     B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc2 = launch_rs<T, OP>(c, a, stream); }));
     return rc2;
   });
+}
+
+extern "C" int b200_reducescatter_multi(b200_comm_t c, const void *const *ins, void *const *outs,
+                                        const size_t *counts, int ntensors, int dtype, int op, void *stream_) {
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op)) ||
+      (rc = check_list(ntensors, ins && outs && counts)))
+    return rc;
+  std::vector<size_t> nbytes(static_cast<size_t>(ntensors));
+  for (int i = 0; i < ntensors; ++i) nbytes[i] = counts[i] * es;
+  if ((rc = check_list_ptrs(outs, nbytes.data(), ntensors)) ||
+      (rc = check_list_rank_ptrs(ins, nbytes.data(), ntensors, c->world, "input")))
+    return rc;
+  if (ntensors == 0) return B200_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  const int n = c->world;
+  if (n == 1) {
+    for (int i = 0; i < ntensors; ++i)
+      if (nbytes[i] && outs[i] != ins[i])
+        B200_CHECK_CUDA(cudaMemcpyAsync(outs[i], ins[i], nbytes[i], cudaMemcpyDeviceToDevice, stream));
+    return B200_OK;
+  }
+  void (*kernel)(DevComm, const RSTableArgs) = nullptr;
+  B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatter_table_kernel<T, OP>; }));
+  // One launch per window of each table's stream of output units; the n sub-slots of a window
+  // fill at most one staging slot.
+  RSTableArgs a{};
+  a.staging_bytes = c->staging_bytes;
+  return for_each_window(
+      a.t, outs, nbytes.data(), ntensors, c->staging_bytes / (16 * size_t(n)),
+      [&](int k, int i) {
+        for (int q = 0; q < n; ++q) a.ins[k][q] = static_cast<const char *>(ins[size_t(i) * n + q]);
+      },
+      [&](size_t done, size_t units) -> int {
+        a.u0 = done;
+        a.units = units;
+        int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+        kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
+        B200_LAUNCH_CHECK(c);
+        return B200_OK;
+      });
 }
 
 extern "C" int b200_reduce(b200_comm_t c, void *buf, size_t count, int dtype, int op, int root,

@@ -1,6 +1,7 @@
 // tensor_table.cuh — tensor lists as one packed stream of 16-byte units, shared by the list
-// point-to-point calls (p2p.cu: b200_send_multi / b200_recv_multi / b200_get_multi) and the list
-// broadcast (copy_ops.cu: b200_broadcast_multi).
+// point-to-point calls (p2p.cu: b200_send_multi / b200_recv_multi / b200_get_multi), the list
+// broadcast and all-gather (copy_ops.cu: b200_broadcast_multi, b200_allgather_multi) and the list
+// reduce-scatter (reduce_ops.cu: b200_reducescatter_multi).
 //
 // A table's tensors form ONE packed stream: tensor i occupies 16-byte units [ustart[i], ustart[i+1])
 // with ustart[i+1] = ustart[i] + ceil(nbytes[i] / 16), so no unit mixes two tensors.  The padding of
@@ -65,6 +66,26 @@ inline int check_list_ptrs(const void *const *ptrs, const size_t *nbytes, int nt
   return B200_OK;
 }
 
+// The per-rank pointers of a gathered or scattered list: ptrs[i * world + p] belongs to entry i
+// (nbytes[i] bytes) and rank p.
+inline int check_list_rank_ptrs(const void *const *ptrs, const size_t *nbytes, int ntensors, int world,
+                                const char *what) {
+  for (int i = 0; i < ntensors; ++i)
+    for (int p = 0; p < world; ++p)
+      if (nbytes[i] && !ptrs[size_t(i) * world + p]) {
+        set_error("%s %d of tensor %d is null but has %zu bytes", what, p, i, nbytes[i]);
+        return B200_ERR_INVALID;
+      }
+  return B200_OK;
+}
+
+// Kernel parameters are limited to 32764 bytes on sm_90 (CUDA >= 12.1); a list kernel takes the
+// communicator and its table arguments.
+template <typename Args>
+constexpr bool fits_param_space() {
+  return sizeof(DevComm) + sizeof(Args) <= 32764;
+}
+
 // Runs launch(lo, hi) over [0, ntensors) cut into runs of at most kP2PTableMax non-empty entries, in
 // list order.  The cut depends on the size list alone, so every rank cuts alike.
 template <typename Fn>
@@ -95,6 +116,24 @@ inline bool fill_table(P2PTable &t, void *const *bufs, const size_t *nbytes, int
     whole_aligned = whole_aligned && is_aligned16(bufs[i]) && (nbytes[i] & 15) == 0;
   }
   return whole_aligned;
+}
+
+// The launch loop of the list collectives (b200_broadcast_multi, b200_allgather_multi,
+// b200_reducescatter_multi): each table of for_each_table is packed into t, pack(k, i) adds what the
+// kernel needs beyond the P2PTable for packed entry k (list entry i), and launch(u0, units) then runs
+// once per window of at most window_units units of the table's stream, in order.  The windows depend
+// on the size list and window_units alone, so every rank makes the same launches.  Entries of t past
+// t.count keep stale values of an earlier table; the kernels never read them.
+template <typename Pack, typename Launch>
+inline int for_each_window(P2PTable &t, void *const *bufs, const size_t *nbytes, int ntensors, size_t window_units,
+                           Pack pack, Launch launch) {
+  return for_each_table(nbytes, ntensors, [&](int lo, int hi) -> int {
+    t.count = 0;
+    fill_table(t, bufs, nbytes, lo, hi);
+    for (int i = lo, k = 0; i < hi; ++i)
+      if (nbytes[i]) pack(k++, i);
+    return for_each_piece(t.ustart[t.count], window_units, launch);
+  });
 }
 
 }  // namespace b200

@@ -262,9 +262,49 @@ class B200ProcessGroup(dist.ProcessGroup):
         return self._run(tensors, lambda comm: comm.broadcast_multi([self._contig(t) for t in tensors], root),
                          tensors)
 
+    @staticmethod
+    def _cpu_each(calls):
+        """gloo ops one after another (gloo has no coalesced form of them): the host waits for all
+        but the last, whose work is returned."""
+        work = None
+        for call in calls:
+            if work is not None:
+                work.wait()
+            work = call()
+        return work
+
+    @staticmethod
+    def _by_dtype(outputs, inputs):
+        """[(outputs, inputs)] per dtype of the outputs, in order of first appearance: a list
+        reduce-scatter takes one dtype per call, and every rank passes the same list."""
+        groups = {}
+        for o, i in zip(outputs, inputs):
+            outs, ins = groups.setdefault(o.dtype, ([], []))
+            outs.append(o)
+            ins.append(i)
+        return list(groups.values())
+
+    def _allgather_lists(self, output_lists, inputs) -> B200Work:
+        """output_lists[i][p] receives rank p's inputs[i], in one b200_allgather_multi call; an output
+        list that is not contiguous receives through temporaries and a copy."""
+
+        def fn(comm):
+            lists = [list(outs) if all(o.is_contiguous() for o in outs) else [torch.empty_like(t) for _ in outs]
+                     for outs, t in zip(output_lists, inputs)]
+            comm.allgather_multi(lists, [self._contig(t) for t in inputs])
+            for outs, got in zip(output_lists, lists):
+                for o, s in zip(outs, got):
+                    if o is not s:
+                        o.copy_(s)
+
+        flat = [o for outs in output_lists for o in outs] + list(inputs)
+        return self._run(flat, fn, output_lists)
+
     def allgather(self, output_tensors, input_tensors, opts=None):
         if not self._all_cuda(input_tensors):
             return self._cpu_group().allgather(output_tensors, input_tensors, opts)
+        if len(input_tensors) > 1:
+            return self._allgather_lists(output_tensors, input_tensors)
 
         def fn(comm):
             for outs, t in zip(output_tensors, input_tensors):
@@ -285,17 +325,38 @@ class B200ProcessGroup(dist.ProcessGroup):
         return self._run([output, input],
                          lambda comm: comm.allgather_into(self._contig(output), self._contig(input)), output)
 
-    def allgather_into_tensor_coalesced(self, outputs, inputs, opts=None):
-        def fn(comm):
-            for o, i in zip(outputs, inputs):
-                comm.allgather_into(self._contig(o), self._contig(i))
+    def allgather_coalesced(self, output_lists, input_list, opts=None):
+        """``dist.all_gather_coalesced``: ``output_lists[p][i]`` receives rank p's ``input_list[i]``,
+        in one ``b200_allgather_multi`` call."""
+        if not self._all_cuda(input_list):
+            return self._cpu_group().allgather_coalesced(output_lists, input_list, opts)
+        if len(output_lists) != self._size or any(len(outs) != len(input_list) for outs in output_lists):
+            raise RuntimeError("allgather_coalesced expects world_size output lists, each as long as the input list")
+        return self._allgather_lists([[outs[i] for outs in output_lists] for i in range(len(input_list))],
+                                     input_list)
 
-        return self._run(list(outputs) + list(inputs), fn, outputs)
+    def allgather_into_tensor_coalesced(self, outputs, inputs, opts=None):
+        """The fast path of ``_coalescing_manager`` around ``all_gather_into_tensor`` calls: one
+        ``b200_allgather_multi`` call for the whole block."""
+        if not self._all_cuda(inputs):
+            gloo = self._cpu_group()
+            return self._cpu_each([lambda o=o, i=i: gloo._allgather_base(o, i) for o, i in zip(outputs, inputs)])
+        return self._run(list(outputs) + list(inputs),
+                         lambda comm: comm.allgather_into_multi([self._contig(o) for o in outputs],
+                                                                [self._contig(i) for i in inputs]), outputs)
 
     def reduce_scatter(self, output_tensors, input_tensors, opts=None):
         if not self._all_cuda(output_tensors):
             return self._cpu_group().reduce_scatter(output_tensors, input_tensors, opts)
         op = _op_code(opts.reduceOp) if opts is not None else N.SUM
+        if len(output_tensors) > 1:
+            def fn_multi(comm):
+                for outs, ins in self._by_dtype(output_tensors, input_tensors):
+                    comm.reducescatter_multi([self._contig(o) for o in outs],
+                                             [[self._contig(i) for i in lst] for lst in ins], op)
+
+            flat = list(output_tensors) + [i for ins in input_tensors for i in ins]
+            return self._run(flat, fn_multi, output_tensors)
 
         def fn(comm):
             for out, ins in zip(output_tensors, input_tensors):
@@ -310,11 +371,18 @@ class B200ProcessGroup(dist.ProcessGroup):
                          lambda comm: comm.reducescatter_from(self._contig(output), self._contig(input), op), output)
 
     def reduce_scatter_tensor_coalesced(self, outputs, inputs, opts=None):
+        """The fast path of ``_coalescing_manager`` around ``reduce_scatter_tensor`` calls: one
+        ``b200_reducescatter_multi`` call per dtype, in order of first appearance."""
+        if not self._all_cuda(outputs):
+            gloo = self._cpu_group()
+            rs_opts = opts if opts is not None else dist.ReduceScatterOptions()
+            return self._cpu_each([lambda o=o, i=i: gloo._reduce_scatter_base(o, i, rs_opts) for o, i in
+                                   zip(outputs, inputs)])
         op = _op_code(opts.reduceOp) if opts is not None else N.SUM
 
         def fn(comm):
-            for o, i in zip(outputs, inputs):
-                comm.reducescatter_from(self._contig(o), self._contig(i), op)
+            for outs, ins in self._by_dtype(outputs, inputs):
+                comm.reducescatter_from_multi([self._contig(o) for o in outs], [self._contig(i) for i in ins], op)
 
         return self._run(list(outputs) + list(inputs), fn, outputs)
 

@@ -5,7 +5,8 @@ GPU, launches replayed from CUDA graphs so host launch overhead does not pollute
         [--min 1024 --max 1073741824] [--op allreduce|allgather|reducescatter|broadcast|sendrecv|grad|
                                             grad_rs|grad_rs_unfused|alltoall|alltoall_p2p|
                                             sendrecv_multi|sendrecv_loop|bcast_multi|bcast_loop|
-                                            bcast_coalesced] [--tensors 16,256,resnet50,resnet50_buffers]
+                                            bcast_coalesced|ag_multi|ag_loop|ag_flat|rs_multi|rs_loop|rs_flat]
+        [--tensors 16,256,resnet50,resnet50_buffers]
         [--split uniform|skew|local] [--wire bfloat16]
 
 Prints one line per (size, algo, blocks): us per launch, algbw, busbw (nccl-tests convention).
@@ -22,6 +23,12 @@ the own segment the largest); --split local keeps `size` bytes on the rank and s
 ``bcast_multi`` broadcasts a tensor list from rank 0 with b200_broadcast_multi, ``bcast_loop`` with
 one b200_broadcast per tensor, and ``bcast_coalesced`` the way DDP's buffer sync does through c10d
 today: flatten per dtype, one broadcast per dtype, a copy back into every tensor on the other ranks.
+``ag_multi`` all-gathers a tensor list into rank-major outputs (the all_gather_into_tensor layout)
+with one b200_allgather_multi call, ``ag_loop`` with one allgather_into per tensor (c10d's coalesced
+all-gather before the list call), and ``ag_flat`` the bucket way: copy into one flat buffer, one
+b200_allgather, one multi-tensor copy back into the outputs.  ``rs_multi``, ``rs_loop`` and
+``rs_flat`` are the same three for reduce-scatter (uint8 SUM).  For these six ops the list is one
+rank's part, so every rank holds world_size times it.
 The list comes from --tensors: N equal tensors of size / N bytes, ResNet-50's parameter list or
 ResNet-50's buffers (fp32 and int64).
 """
@@ -102,7 +109,8 @@ def alltoall_p2p(c, r, n, outs, ins, side):
     cur.wait_stream(side)
 
 
-LIST_OPS = ("sendrecv_multi", "sendrecv_loop", "bcast_multi", "bcast_loop", "bcast_coalesced")
+LIST_OPS = ("sendrecv_multi", "sendrecv_loop", "bcast_multi", "bcast_loop", "bcast_coalesced",
+            "ag_multi", "ag_loop", "ag_flat", "rs_multi", "rs_loop", "rs_flat")
 
 
 def tensor_list_specs(recipe, size):
@@ -148,6 +156,27 @@ def bcast_coalesced(c, r, tensors):
         if r != 0:
             for t, f in zip(ts, flat.split([t.numel() for t in ts])):
                 t.view(-1).copy_(f)
+
+
+def ag_flat(c, n, outs, parts, flat_in, flat_out):
+    """The bucket all-gather: copy the list into one flat buffer, one all-gather, one multi-tensor
+    copy of every rank's slice back into the rank-major outputs.  With c = None only the torch
+    kernels run (to load them outside any collective)."""
+    torch.cat(parts, out=flat_in)
+    if c is not None:
+        c.allgather_into(flat_out, flat_in)
+    rows = flat_out.view(n, -1).split([t.numel() for t in parts], dim=1)
+    torch._foreach_copy_([o.view(n, -1) for o in outs], list(rows))
+
+
+def rs_flat(c, n, outs, ins, flat_in, flat_out):
+    """The bucket reduce-scatter: one multi-tensor copy of the rank-major inputs into one rank-major
+    flat buffer, one reduce-scatter, one multi-tensor copy of the result back into the outputs."""
+    rows = flat_in.view(n, -1).split([o.numel() for o in outs], dim=1)
+    torch._foreach_copy_(list(rows), [t.view(n, -1) for t in ins])
+    if c is not None:
+        c.reducescatter_from(flat_out, flat_in, N.SUM)
+    torch._foreach_copy_(outs, list(flat_out.split([o.numel() for o in outs])))
 
 
 def grad_rs_unfused(c, out, grad, wout, scale, wire):
@@ -281,9 +310,21 @@ def main():
             sends = [torch.ones(s, dtype=torch.uint8, device=g.device(0)) for s in sizes]
             recvs = [torch.empty(s, dtype=torch.uint8, device=g.device(1)) for s in sizes]
             lists = [[torch.ones(k, dtype=dt, device=g.device(r)) for k, dt in specs] for r in range(n)]
+            total = sum(sizes)
+            gather = [op for op in list_ops if op[:3] in ("ag_", "rs_")]
+            if gather:
+                # one rank's part: `parts` (inputs of all-gather, outputs of reduce-scatter) and the
+                # rank-major `wholes` (outputs of all-gather, inputs of reduce-scatter)
+                parts = [[torch.ones(s, dtype=torch.uint8, device=g.device(r)) for s in sizes] for r in range(n)]
+                wholes = [[torch.ones(n * s, dtype=torch.uint8, device=g.device(r)) for s in sizes] for r in range(n)]
+                flat_part = [torch.empty(total, dtype=torch.uint8, device=g.device(r)) for r in range(n)]
+                flat_whole = [torch.empty(n * total, dtype=torch.uint8, device=g.device(r)) for r in range(n)]
             for r in range(n):
                 with torch.cuda.device(g.devices[r]):
                     bcast_coalesced(None, r, lists[r])
+                    if gather:
+                        ag_flat(None, n, wholes[r], parts[r], flat_part[r], flat_whole[r])
+                        rs_flat(None, n, parts[r], wholes[r], flat_whole[r], flat_part[r])
             for op in list_ops:
                 if op == "sendrecv_multi":
                     call = lambda c, r: (c.send_multi(sends, 1) if r == 0 else  # noqa: E731
@@ -294,11 +335,22 @@ def main():
                     call = lambda c, r: c.broadcast_multi(lists[r], 0)  # noqa: E731
                 elif op == "bcast_loop":
                     call = lambda c, r: bcast_loop(c, lists[r])  # noqa: E731
+                elif op == "ag_multi":
+                    call = lambda c, r: c.allgather_into_multi(wholes[r], parts[r])  # noqa: E731
+                elif op == "ag_loop":
+                    call = lambda c, r: [c.allgather_into(o, t) for o, t in zip(wholes[r], parts[r])]  # noqa: E731
+                elif op == "ag_flat":
+                    call = lambda c, r: ag_flat(c, n, wholes[r], parts[r], flat_part[r], flat_whole[r])  # noqa: E731
+                elif op == "rs_multi":
+                    call = lambda c, r: c.reducescatter_from_multi(parts[r], wholes[r], N.SUM)  # noqa: E731
+                elif op == "rs_loop":
+                    call = lambda c, r: [c.reducescatter_from(o, t, N.SUM) for o, t in zip(parts[r], wholes[r])]  # noqa: E731
+                elif op == "rs_flat":
+                    call = lambda c, r: rs_flat(c, n, parts[r], wholes[r], flat_whole[r], flat_part[r])  # noqa: E731
                 else:
                     call = lambda c, r: bcast_coalesced(c, r, lists[r])  # noqa: E731
                 torch.cuda.synchronize()
                 us = time_graphs(g, call, iters)
-                total = sum(sizes)
                 print(f"{op} {total:>11d} B  tensors={recipe}({len(sizes)}) {us:10.2f} us  "
                       f"algbw={total / us / 1e3:8.1f} GB/s", flush=True)
         size *= args.step
