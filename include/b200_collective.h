@@ -207,7 +207,9 @@ int b200_alltoall(b200_comm_t comm, const void *const *ins, const size_t *send_c
  * its same-GPU restriction): copies [src_heap_offset, +nbytes) of rank `src_rank`'s symmetric heap
  * into `dst` with a kernel that runs on THIS rank only.  The caller orders it after the owner's
  * writes (an interprocess event in the RDT transport).  b200_symm_base returns this rank's heap
- * base and size, so that an address inside it can be turned into the offset a peer passes here. */
+ * base and size, so that an address inside it can be turned into the offset a peer passes here.  A
+ * range outside the heap, or a NULL destination with a non-zero size, refuses the call before
+ * anything is launched. */
 int b200_symm_base(b200_comm_t comm, void **base, size_t *bytes);
 int b200_get(b200_comm_t comm, void *dst, int src_rank, size_t src_heap_offset, size_t nbytes, void *stream);
 

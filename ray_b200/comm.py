@@ -510,6 +510,8 @@ class B200Comm:
         """Pull ``dst.nbytes`` bytes from ``src_rank``'s symmetric heap into ``dst``; only this rank
         runs a kernel."""
         _check_cuda_contiguous(dst)
+        if src_heap_offset < 0:
+            raise ValueError("range outside the symmetric heap")
         N.check(self._lib.b200_get(self._h, dst.data_ptr(), int(src_rank), int(src_heap_offset),
                                    dst.numel() * dst.element_size(),
                                    stream.cuda_stream if stream is not None else self._stream()))

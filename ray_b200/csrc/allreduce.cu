@@ -298,6 +298,7 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
     if (c->world == 2) pipe_variant = PIPE_PULL;
     else if (c->mc_active && nvls_capable(dtype, op)) pipe_variant = PIPE_NVLS;
     else if (algo == B200_ALGO_PIPE) pipe_variant = PIPE_PEER;  // AUTO without NVLS keeps the two-shot kernel
+    if (algo == B200_ALGO_AUTO && pipe_variant >= 0 && !pipe_runs(c, PipeVariant(pipe_variant))) pipe_variant = -1;
   } else if (algo == B200_ALGO_PIPE) {
     set_error("the pipelined all-reduce needs 16-byte aligned operands outside the symmetric heap "
               "and a size that is a multiple of 16 bytes");

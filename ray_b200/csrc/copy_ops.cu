@@ -235,7 +235,7 @@ extern "C" int b200_allgather(b200_comm_t c, const void *in, void *const *outs, 
   // into the caller's output tensors, allreduce_pipe.cu).
   bool aligned = is_aligned16(in) && (total & 15) == 0 && pipe_fits(c);
   for (int p = 0; p < c->world; ++p) aligned = aligned && is_aligned16(outs[p]);
-  if (aligned && ag_pull_pays_off(c, total)) {
+  if (aligned && ag_pull_pays_off(c, total) && pipe_runs(c, PIPE_GATHER)) {
     return for_each_piece(total, pipe_plan(c, PIPE_GATHER).max_bytes, [&](size_t done, size_t nbytes) {
       char *o[kMaxRanks] = {};
       for (int p = 0; p < c->world; ++p) o[p] = static_cast<char *>(outs[p]) + done;

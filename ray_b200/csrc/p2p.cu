@@ -727,7 +727,7 @@ extern "C" int b200_symm_base(b200_comm_t c, void **base, size_t *bytes) {
 extern "C" int b200_get(b200_comm_t c, void *dst, int src_rank, size_t src_heap_offset, size_t nbytes, void *stream_) {
   int rc;
   if ((rc = check_usable(c)) || (rc = check_rank(c, src_rank, "source"))) return rc;
-  if (src_heap_offset + nbytes > c->heap_bytes) {
+  if (src_heap_offset > c->heap_bytes || nbytes > c->heap_bytes - src_heap_offset) {
     set_error("[%zu, %zu) is outside the %zu-byte symmetric heap", src_heap_offset, src_heap_offset + nbytes,
               c->heap_bytes);
     return B200_ERR_INVALID;

@@ -140,6 +140,11 @@ inline PipePlan pipe_plan(const b200_comm *c, PipeVariant variant) {
   return p;
 }
 
+// An automatic choice takes a pipelined kernel only when the grid cap leaves it a worker CTA; below
+// that the phase-by-phase kernels, which run on any grid, take the message.  An explicit
+// B200_ALGO_PIPE is refused instead.  The cap is the same on every rank, so all ranks choose alike.
+inline bool pipe_runs(const b200_comm *c, PipeVariant variant) { return pipe_plan(c, variant).work_ctas >= 1; }
+
 // ---- all-gather, broadcast, gradient all-reduce ----------------------------------------------
 
 // Per-rank size from which an aligned all-gather takes the pull kernel (B200_PARAM_AG_PULL_MIN_BYTES;
