@@ -237,6 +237,28 @@ int b200_recv_multi(b200_comm_t comm, void *const *bufs, const size_t *nbytes, i
 int b200_get_multi(b200_comm_t comm, void *const *dsts, int src_rank, const size_t *src_heap_offsets,
                    const size_t *nbytes, int ntensors, void *stream);
 
+/* A batch of point-to-point operations in ONE launch (ncclGroupStart/End of sends and receives).
+ * Op i sends (is_send[i] != 0) or receives nbytes[i] bytes at bufs[i] to / from rank peers[i]; the
+ * arrays are host arrays of nops entries.  Wire identity: each op is exactly the message b200_send /
+ * b200_recv would make for its buffer (same chunking and sub-rings, same persistent sequence
+ * numbers), so it pairs with a plain b200_send / b200_recv on the peer or with an op of the peer's
+ * batch, in any mix, and interleaves in stream order with every other send / recv on the pair.  It
+ * does NOT pair with a b200_alltoall segment or a b200_send_multi / b200_recv_multi message, whose
+ * wire differs.  Order: ops to the same (peer, direction) are consecutive messages in list order;
+ * different (peer, direction) pairs progress concurrently, with no order implied between them.  So
+ * a bidirectional or ring exchange of messages larger than the inbox completes in one batch, where
+ * a send queued ahead of its matching receive would wait for it.  Each side picks ld/st or the
+ * bulk-copy unit per op exactly as b200_send / b200_recv do.  A zero-size op moves nothing and its
+ * pointer may be NULL; a batch whose ops are all empty launches nothing.  Refused calls launch
+ * nothing and return B200_ERR_INVALID: nops < 0 or > B200_P2P_TABLE_MAX (a larger batch is not
+ * split, since separate launches could deadlock again), NULL arrays with nops > 0, a peer out of
+ * range or this rank, a NULL pointer with a non-zero size, and a grid cap (b200_comm_set_blocks)
+ * below 2 * (world_size - 1) -- checked against the world size, so every rank refuses together.
+ * The op table is a kernel parameter, so the call can be captured in a CUDA graph.  Counterpart of
+ * ncclSend / ncclRecv between ncclGroupStart and ncclGroupEnd (c10d's batch_isend_irecv). */
+int b200_p2p_batch(b200_comm_t comm, void *const *bufs, const size_t *nbytes, const int *peers,
+                   const int *is_send, int nops, void *stream);
+
 /* In-place broadcast of a tensor LIST from root: bufs[i] (nbytes[i] bytes) on every rank receives
  * root's bufs[i].  Sizes are in BYTES, so one list may mix dtypes; every rank passes the same size
  * sequence.  A zero-size entry moves nothing and its pointer may be NULL.  Layout: the packed

@@ -98,6 +98,8 @@ SIGNATURES = {
     "b200_recv_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, c_int, c_void_p]),
     "b200_get_multi": (c_int, [c_void_p, POINTER(c_void_p), c_int, POINTER(c_size_t), POINTER(c_size_t), c_int,
                                c_void_p]),
+    "b200_p2p_batch": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_int), POINTER(c_int), c_int,
+                               c_void_p]),
     "b200_broadcast_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, c_int, c_void_p]),
     "b200_allgather_multi": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(c_void_p),
                                      c_void_p]),

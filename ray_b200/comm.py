@@ -474,6 +474,29 @@ class B200Comm:
         N.check(self._lib.b200_recv_multi(self._h, ptrs, sizes, len(tensors), int(peer),
                                           stream.cuda_stream if stream is not None else self._stream()))
 
+    def p2p_batch(self, ops: Sequence, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Run a list of sends and receives as one launch (``ncclGroupStart/End`` of sends and
+        receives).  ``ops`` holds ``(is_send, tensor, peer)`` triples; tensors are contiguous CUDA
+        tensors of any dtype and move as raw bytes.  Each op is the message ``send`` / ``recv`` would
+        make, so it pairs with a plain ``send`` / ``recv`` on the peer or with an op of the peer's
+        batch; ops to one (peer, direction) are consecutive messages in list order.  A bidirectional
+        or ring exchange larger than the inbox completes here, where plain calls in the wrong order
+        would wait on each other.  At most ``N.P2P_TABLE_MAX`` ops per batch."""
+        ops = list(ops)
+        if not ops:
+            return
+        n = len(ops)
+        bufs, sizes = (ctypes.c_void_p * n)(), (ctypes.c_size_t * n)()
+        peers, sends = (ctypes.c_int * n)(), (ctypes.c_int * n)()
+        for i, (is_send, t, peer) in enumerate(ops):
+            _check_cuda_contiguous(t, f"tensor {i}")
+            bufs[i] = t.data_ptr()
+            sizes[i] = t.numel() * t.element_size()
+            peers[i] = int(peer)
+            sends[i] = 1 if is_send else 0
+        N.check(self._lib.b200_p2p_batch(self._h, bufs, sizes, peers, sends, n,
+                                         stream.cuda_stream if stream is not None else self._stream()))
+
     def send_ptr(self, ptr: int, nbytes: int, peer: int, stream: Optional[torch.cuda.Stream] = None) -> None:
         """send() from a raw device-visible address (e.g. pinned host memory under unified
         addressing: the Compiled-Graph channel keeps its metadata header there)."""

@@ -108,6 +108,16 @@ __device__ __forceinline__ BulkRing bulk_ring_init(char *dyn_smem) {
   return r;
 }
 
+// Thread 0 ends the mbarrier objects of a drained ring (every load waited for, every store
+// completed), so that a later bulk_ring_init on the same CTA initialises fresh memory: mbarrier.init
+// on a location that holds a valid mbarrier object is undefined in PTX.
+__device__ __forceinline__ void bulk_ring_inval(char *dyn_smem) {
+  if (threadIdx.x != 0) return;
+  const uint32_t bars = smem_u32(dyn_smem) + kBulkStages * kBulkTile;
+  for (int s = 0; s < kBulkStages; ++s)
+    asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(bars + 8 * s) : "memory");
+}
+
 // ---------------------------------------------------------------------------
 // Segment engine.  One thread issues every tile, and a single thread retires a dependent
 // instruction every ~5 cycles, so the per-tile instruction count IS the throughput limit

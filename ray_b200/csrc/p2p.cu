@@ -27,7 +27,9 @@
 // Both are thin wrappers around p2p_ldst_ring / p2p_bulk_ring (one CTA's share of a message), which
 // alltoall_kernel also runs: all 2(n-1) transfers of an all-to-all as roles of one grid, each role
 // picking its own copy mechanism.  The same two functions move a table of tensors as one message
-// (p2p_table_kernel / p2p_bulk_table_kernel: b200_send_multi / b200_recv_multi).
+// (p2p_table_kernel / p2p_bulk_table_kernel: b200_send_multi / b200_recv_multi), and run a batch of
+// sends and receives, each on the plain send / recv wire, as one grid (p2p_batch_kernel:
+// b200_p2p_batch).
 #include <type_traits>
 
 #include "bulk_copy.cuh"
@@ -449,6 +451,81 @@ __global__ void __launch_bounds__(kThreads, 1) alltoall_kernel(DevComm c, A2AArg
 }
 
 // ---------------------------------------------------------------------------
+// grouped point-to-point (b200_p2p_batch): a list of sends and receives as ONE co-resident grid.
+// Op i is the very message b200_send / b200_recv would make for its buffer -- p2p_plan's chunk and
+// R rings, on the same sub-rings and persistent sequence numbers -- so it pairs with a plain send /
+// recv on the peer or with an op of the peer's batch, in any mix.
+//
+// Each (peer, direction) present is a role of G CTAs (p2p_batch_ctas), holding its ops in list
+// order.  Sub-ring r of every op of the role belongs to CTA r mod G, which runs exactly what CTA r of
+// the standalone p2p_kernel / p2p_bulk_kernel would, for each of its (op, sub-ring) pairs in
+// lexicographic order.  One sub-ring's messages therefore stay serialised on one CTA, in order.
+//
+// Why folding cannot deadlock against any peer: number the messages of a directed pair m = 0, 1, ...
+// in stream order (the same numbering on both sides), and consider the smallest (m, r) that some
+// side has not finished.  Every CTA of either side serving it has finished all its smaller items, so
+// it is serving (m, r) right now -- the grid is co-resident, and a plain kernel runs only once the
+// stream reached message m.  A sender of (m, r) waits only for acks of earlier chunks of sub-ring r,
+// which the receiver of (m, r) or of an earlier message on r gives; a receiver waits only for chunks
+// of (m, r).  So both ends of (m, r) run and it completes: a waiting CTA only ever waits on a
+// lexicographically earlier-or-equal (m, r) of the other side, whatever G each side chose.
+// ---------------------------------------------------------------------------
+struct P2PBatchOp {
+  char *buf;
+  size_t nbytes;
+  size_t chunk;  // p2p_plan's, the same on both sides
+  int rings;     // R: p2p_plan's sub-rings for nbytes
+  int bulk;      // this side moves the op with the bulk-copy unit
+};
+
+struct P2PBatchRole {
+  int peer;
+  int send;
+  int first;   // first CTA of the role in the grid
+  int G;       // CTAs of the role
+  int lo, hi;  // its ops: op[lo, hi), in list order
+};
+
+struct P2PBatchArgs {
+  P2PBatchRole role[2 * (kMaxRanks - 1)];
+  int nroles;
+  P2PBatchOp op[kP2PTableMax];  // grouped by role
+};
+static_assert(fits_param_space<P2PBatchArgs>(), "p2p batch table exceeds the kernel parameter space");
+
+// Called by every thread between two ring calls of one CTA.  The barrier orders the previous call's
+// write-back of the sequence word (thread 0) before the next call reads it (every thread), and its
+// shared words before their reset.  Returns whether a wait was abandoned: the ring functions record
+// an abort or a watchdog expiry in the sticky status word, from thread 0, before they return.
+__device__ __forceinline__ bool p2p_batch_gave_up(const DevComm &c) {
+  return __syncthreads_or(threadIdx.x == 0 && *reinterpret_cast<volatile int32_t *>(&c.st->status) != 0) != 0;
+}
+
+__global__ void __launch_bounds__(kThreads, 1) p2p_batch_kernel(DevComm c, const __grid_constant__ P2PBatchArgs a) {
+  extern __shared__ __align__(128) char dyn_smem[];
+  const int cta = int(blockIdx.x);
+  int i = 0;
+  while (i + 1 < a.nroles && cta >= a.role[i + 1].first) ++i;
+  const P2PBatchRole &r = a.role[i];
+  const int b = cta - r.first;
+  for (int k = r.lo; k < r.hi; ++k) {
+    const P2PBatchOp &o = a.op[k];
+    for (int ring = b; ring < o.rings; ring += r.G) {
+      if (o.bulk) {
+        if (r.send) p2p_bulk_ring<true>(c, r.peer, ring, o.rings, o.buf, o.nbytes, o.chunk, dyn_smem, [](int, int) {});
+        else p2p_bulk_ring<false>(c, r.peer, ring, o.rings, o.buf, o.nbytes, o.chunk, dyn_smem, [](int, int) {});
+        bulk_ring_inval(dyn_smem);
+      } else if (r.send) {
+        p2p_ldst_ring<true>(c, r.peer, ring, o.rings, o.buf, o.nbytes, o.chunk);
+      } else {
+        p2p_ldst_ring<false>(c, r.peer, ring, o.rings, o.buf, o.nbytes, o.chunk);
+      }
+      if (p2p_batch_gave_up(c)) return;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
 // one-sided get: the receiver pulls [src_off, src_off + nbytes) of a PEER's symmetric heap into a
 // local tensor.  No kernel runs on the owner of the data (RDT's one-sided contract,
 // experimental/rdt/cuda_ipc_transport.py:57-186); ordering against the owner's writes is the
@@ -592,6 +669,66 @@ static int p2p_multi_common(b200_comm *c, void *const *bufs, const size_t *nbyte
   });
 }
 
+static int p2p_batch(b200_comm *c, void *const *bufs, const size_t *nbytes, const int *peers, const int *is_send,
+                     int nops, cudaStream_t stream) {
+  int rc;
+  if ((rc = check_usable(c)) || (rc = check_list(nops, bufs && nbytes && peers && is_send))) return rc;
+  if (nops > kP2PTableMax) {
+    set_error("%d operations in one batch; at most %d fit one launch", nops, kP2PTableMax);
+    return B200_ERR_INVALID;
+  }
+  for (int i = 0; i < nops; ++i) {
+    if ((rc = check_rank(c, peers[i], "peer"))) return rc;
+    if (peers[i] == c->rank) {
+      set_error("operation %d: peer rank %d is this rank", i, peers[i]);
+      return B200_ERR_INVALID;
+    }
+  }
+  if ((rc = check_list_ptrs(bufs, nbytes, nops))) return rc;
+  // Every role needs a CTA.  Checked against the world size rather than this batch's ops, so all
+  // ranks refuse together instead of one refusing while its peers wait for it.
+  const int n = c->world, cap = a2a_grid_cap(c);
+  if (cap < 2 * (n - 1)) {
+    set_error("a p2p batch needs %d co-resident CTAs at world size %d but the grid is capped at %d "
+              "(b200_comm_set_blocks)", 2 * (n - 1), n, cap);
+    return B200_ERR_INVALID;
+  }
+  P2PBatchArgs a{};
+  int nops_live = 0, roles = 0, max_rings[2 * (kMaxRanks - 1)] = {};
+  bool any_bulk = false;
+  for (int send = 1; send >= 0; --send) {
+    for (int peer = 0; peer < n; ++peer) {
+      const int lo = nops_live;
+      for (int i = 0; i < nops; ++i) {
+        if (!nbytes[i] || peers[i] != peer || (is_send[i] != 0) != (send != 0)) continue;
+        // exactly what b200_send / b200_recv would launch for this buffer
+        const P2PPlan p = p2p_plan(c, bufs[i], nbytes[i]);
+        a.op[nops_live++] = P2PBatchOp{static_cast<char *>(bufs[i]), nbytes[i], p.chunk, p.rings, p.bulk};
+        any_bulk = any_bulk || p.bulk;
+        if (p.rings > max_rings[roles]) max_rings[roles] = p.rings;
+      }
+      if (nops_live > lo) a.role[roles++] = P2PBatchRole{peer, send, 0, 0, lo, nops_live};
+    }
+  }
+  if (roles == 0) return B200_OK;
+  int grid = 0;
+  for (int i = 0; i < roles; ++i) {
+    a.role[i].first = grid;
+    a.role[i].G = p2p_batch_ctas(cap, roles, max_rings[i]);
+    grid += a.role[i].G;  // <= cap: roles <= 2(n-1) <= cap, and G <= max(1, cap / roles)
+  }
+  a.nroles = roles;
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  if (any_bulk) {
+    if ((rc = set_dyn_smem(c->device, reinterpret_cast<const void *>(p2p_batch_kernel)))) return rc;
+    p2p_batch_kernel<<<grid, kThreads, kBulkSmemBytes, stream>>>(c->dev(), a);
+  } else {
+    p2p_batch_kernel<<<grid, kThreads, 0, stream>>>(c->dev(), a);
+  }
+  B200_LAUNCH_CHECK(c);
+  return B200_OK;
+}
+
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
 const void *p2p_module_anchor() { return reinterpret_cast<const void *>(&get_bulk_kernel); }
 
@@ -616,6 +753,11 @@ extern "C" int b200_send_multi(b200_comm_t c, const void *const *bufs, const siz
 extern "C" int b200_recv_multi(b200_comm_t c, void *const *bufs, const size_t *nbytes, int ntensors, int peer,
                                void *stream) {
   return p2p_multi_common(c, bufs, nbytes, ntensors, peer, static_cast<cudaStream_t>(stream), false);
+}
+
+extern "C" int b200_p2p_batch(b200_comm_t c, void *const *bufs, const size_t *nbytes, const int *peers,
+                              const int *is_send, int nops, void *stream) {
+  return p2p_batch(c, bufs, nbytes, peers, is_send, nops, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200_alltoall(b200_comm_t c, const void *const *ins, const size_t *send_counts, void *const *outs,

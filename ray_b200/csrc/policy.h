@@ -244,6 +244,17 @@ inline int a2a_ring_cap(const b200_comm *c, int cap) {
   return k < 1 ? 1 : (k > kP2PRings ? kP2PRings : k);
 }
 
+// CTAs of one (peer, direction) role of b200_p2p_batch: the roles present share the co-resident grid,
+// and a role never takes more CTAs than its largest op has sub-rings.  A local choice: each op keeps
+// p2p_plan's rings on the wire, and a role with fewer CTAs than rings folds several sub-rings onto
+// one CTA, so the peer may choose differently.
+inline int p2p_batch_ctas(int cap, int roles, int max_rings) {
+  int g = cap / roles;
+  if (g < 1) g = 1;
+  if (g > max_rings) g = max_rings;
+  return g > kP2PRings ? kP2PRings : g;
+}
+
 // A large own segment gets copy-only CTAs, one per 64 KiB: a local copy of MiBs next to small
 // remote messages would otherwise crawl through the few role CTAs.
 inline size_t a2a_own_ctas(size_t own_bytes) { return (own_bytes + (size_t(64) << 10) - 1) / (size_t(64) << 10); }

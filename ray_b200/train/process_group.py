@@ -129,6 +129,42 @@ class B200Work(dist._Work):
         return self._result if isinstance(self._result, list) else [self._result]
 
 
+class _CoalescedP2PWork(dist._Work):
+    """What ``send`` / ``recv`` return inside a coalescing block: it completes with the block's one
+    batch launch, so it can only be waited for once the block has ended."""
+
+    def __init__(self, result):
+        super().__init__()
+        self._result = result
+        self._batch: Optional[B200Work] = None
+
+    def _work(self) -> B200Work:
+        if self._batch is None:
+            raise RuntimeError("this send / recv runs when its coalescing block ends; wait for it after the block")
+        return self._batch
+
+    def wait(self, timeout=None) -> bool:
+        return self._work().wait(timeout)
+
+    def synchronize(self) -> None:
+        self.wait()
+
+    def is_completed(self) -> bool:
+        return self._batch is not None and self._batch.is_completed()
+
+    def is_success(self) -> bool:
+        return self._work().is_success()
+
+    def exception(self):
+        return self._batch.exception() if self._batch is not None else None
+
+    def get_future(self):
+        return self._work().get_future()
+
+    def result(self):
+        return self._result
+
+
 class B200ProcessGroup(dist.ProcessGroup):
     """One rank's c10d process group.  CUDA tensors go to the B200 kernels; CPU tensors (rare:
     object collectives, barriers issued before any GPU work) go to an internal gloo group."""
@@ -411,6 +447,8 @@ class B200ProcessGroup(dist.ProcessGroup):
     def send(self, tensors, dst_rank, tag=0):
         if not self._all_cuda(tensors):
             return self._cpu_group().send(tensors, dst_rank, tag)
+        if self._p2p_block is not None:
+            return self._defer_p2p(True, tensors, dst_rank)
 
         def fn(comm):
             for t in tensors:
@@ -421,12 +459,49 @@ class B200ProcessGroup(dist.ProcessGroup):
     def recv(self, tensors, src_rank, tag=0):
         if not self._all_cuda(tensors):
             return self._cpu_group().recv(tensors, src_rank, tag)
+        if self._p2p_block is not None:
+            return self._defer_p2p(False, tensors, src_rank)
 
         def fn(comm):
             for t in tensors:
                 comm.recv(self._contig(t), src_rank)
 
         return self._run(tensors, fn, tensors)
+
+    # ------------------------------------------------------------------ grouped point-to-point
+    #: (is_send, tensor, peer) of the CUDA sends / receives recorded since _start_coalescing, and
+    #: their Work handles; None outside a coalescing block
+    _p2p_block = None
+
+    def _defer_p2p(self, is_send: bool, tensors, peer: int) -> "_CoalescedP2PWork":
+        ops, works = self._p2p_block
+        ops.extend((is_send, self._contig(t), peer) for t in tensors)
+        work = _CoalescedP2PWork(tensors)
+        works.append(work)
+        return work
+
+    def _start_coalescing(self, device):  # noqa: D401 - c10d virtual, called by dist._coalescing_manager
+        """Open a coalescing block: CUDA sends and receives are recorded until ``_end_coalescing``
+        issues them as one ``b200_p2p_batch`` launch (``ncclGroupStart``).  CPU tensors still go to
+        gloo at once, and other ops run as usual: torch issues its coalesced collectives itself."""
+        if self._p2p_block is not None:
+            raise RuntimeError("b200 process group: a coalescing block is already open")
+        self._p2p_block = ([], [])
+
+    def _end_coalescing(self, device):
+        """Close the block (``ncclGroupEnd``): every recorded send and receive runs as one launch,
+        whose Work is returned; the Work each ``send`` / ``recv`` returned completes with it."""
+        block, self._p2p_block = self._p2p_block, None
+        if block is None:
+            raise RuntimeError("b200 process group: no coalescing block is open")
+        ops, works = block
+        if not ops:
+            return None
+        tensors = [t for _, t, _ in ops]
+        work = self._run(tensors, lambda comm: comm.p2p_batch(ops), tensors)
+        for w in works:
+            w._batch = work
+        return work
 
     # ------------------------------------------------------------------ rooted / all-to-all ops
     # gather, scatter and both all-to-all forms are one b200_alltoall launch each
@@ -520,6 +595,25 @@ class B200ProcessGroup(dist.ProcessGroup):
             self.shutdown()
         except Exception:
             pass
+
+
+def batch_isend_irecv(p2p_op_list):
+    """Drop-in for ``dist.batch_isend_irecv`` that pipeline-parallel and ring-exchange code must call
+    on the b200 backend.  torch coalesces the list only for a plain ``ProcessGroup``; on a b200 group
+    it would issue one send or receive after another, and an exchange whose messages exceed the
+    receiver's inbox would then wait forever.  Here a list of CUDA tensors on a b200 group runs inside
+    ``dist._coalescing_manager`` -- torch's own NCCL branch -- as one ``b200_p2p_batch`` launch, and
+    the one Work of that launch is returned.  Any other list goes to ``dist.batch_isend_irecv``."""
+    if p2p_op_list:
+        dist.distributed_c10d._check_p2p_op_list(p2p_op_list)
+        group = p2p_op_list[0].group or dist.distributed_c10d._get_default_group()
+        if isinstance(group, B200ProcessGroup) and all(op.tensor.is_cuda for op in p2p_op_list):
+            with dist._coalescing_manager(group, p2p_op_list[0].tensor.device, async_ops=True) as cm:
+                for op in p2p_op_list:
+                    peer = {"group_dst" if op.op is dist.isend else "group_src": op.group_peer}
+                    op.op(op.tensor, group=op.group, tag=op.tag, **peer)
+            return cm.works
+    return dist.batch_isend_irecv(p2p_op_list)
 
 
 _registered = False

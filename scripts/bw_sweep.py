@@ -5,7 +5,8 @@ GPU, launches replayed from CUDA graphs so host launch overhead does not pollute
         [--min 1024 --max 1073741824] [--op allreduce|allgather|reducescatter|broadcast|sendrecv|grad|
                                             grad_rs|grad_rs_unfused|alltoall|alltoall_p2p|
                                             sendrecv_multi|sendrecv_loop|bcast_multi|bcast_loop|
-                                            bcast_coalesced|ag_multi|ag_loop|ag_flat|rs_multi|rs_loop|rs_flat]
+                                            bcast_coalesced|ag_multi|ag_loop|ag_flat|rs_multi|rs_loop|rs_flat|
+                                            exchange_batch|exchange_ordered|ring_batch|ring_ordered]
         [--tensors 16,256,resnet50,resnet50_buffers]
         [--split uniform|skew|local] [--wire bfloat16]
 
@@ -31,6 +32,10 @@ b200_allgather, one multi-tensor copy back into the outputs.  ``rs_multi``, ``rs
 rank's part, so every rank holds world_size times it.
 The list comes from --tensors: N equal tensors of size / N bytes, ResNet-50's parameter list or
 ResNet-50's buffers (fp32 and int64).
+``exchange_batch`` is a two-rank bidirectional exchange of `size` bytes per direction, both directions
+as one b200_p2p_batch per rank; ``exchange_ordered`` is the same exchange as plain send / recv in an
+order that cannot wait on itself (even ranks send first, odd ranks receive first).  ``ring_batch`` and
+``ring_ordered`` are the same with every rank sending to r+1 and receiving from r-1 (world >= 3).
 """
 import argparse
 import os
@@ -107,6 +112,22 @@ def alltoall_p2p(c, r, n, outs, ins, side):
             c.recv(outs[frm], frm, stream=side)
     outs[r].copy_(ins[r])
     cur.wait_stream(side)
+
+
+def exchange(c, r, k, src, dst, batch):
+    """Ranks [0, k) send `src` to r+1 and receive `dst` from r-1 (mod k): one batch, or plain calls with
+    even ranks sending first and odd ranks receiving first."""
+    if r >= k:
+        return
+    nxt, prv = (r + 1) % k, (r - 1) % k
+    if batch:
+        c.p2p_batch([(True, src, nxt), (False, dst, prv)])
+    elif r % 2 == 0:
+        c.send(src, nxt)
+        c.recv(dst, prv)
+    else:
+        c.recv(dst, prv)
+        c.send(src, nxt)
 
 
 LIST_OPS = ("sendrecv_multi", "sendrecv_loop", "bcast_multi", "bcast_loop", "bcast_coalesced",
@@ -291,6 +312,14 @@ def main():
                         else:
                             call = lambda c, r: alltoall_p2p(c, r, n, outs[r], ins[r], side[r])  # noqa: E731
                         factor = (n - 1) / n  # nccl-tests all-to-all: busbw = algbw * (n-1)/n
+                    elif op in ("exchange_batch", "exchange_ordered", "ring_batch", "ring_ordered"):
+                        k = n if op.startswith("ring") else 2
+                        if k < 3 and op.startswith("ring"):
+                            raise SystemExit(f"{op} needs --world 3 or more")
+                        dsts = [torch.empty(numel, dtype=dtype, device=g.device(r)) for r in range(n)]
+                        batch = op.endswith("batch")
+                        call = lambda c, r: exchange(c, r, k, xs[r], dsts[r], batch)  # noqa: E731
+                        factor = 1.0  # algbw: bytes one rank sends (and receives) per launch sequence
                     else:
                         raise SystemExit(f"unknown op {op}")
                     torch.cuda.synchronize()
