@@ -170,6 +170,44 @@ int b200_allgather(b200_comm_t comm, const void *in, void *const *outs, size_t c
 int b200_reducescatter(b200_comm_t comm, const void *const *ins, void *out, size_t count,
                        int dtype, int op, void *stream);
 
+/* All-gather with a size per rank.  counts: host array of world_size element counts, the same on
+ * every rank.  outs[p] (counts[p] elements) receives rank p's `in` (counts[this rank] elements).
+ * A zero count moves nothing, and its pointer may be NULL; if all counts are zero nothing is
+ * launched.  When all counts are equal the call is exactly b200_allgather: it delegates, so it
+ * makes the same launches (the pull kernel for large aligned parts included).  The only overlap
+ * allowed is the in-place form, outs[this rank] == in.  World size 1: cudaMemcpyAsync when not in
+ * place, no kernel.  Launches: every part is cut into windows of W = staging_bytes / 16 units of 16
+ * bytes; window w covers units [w * W, (w + 1) * W) of every part, so launches = ceil(max_p U_p / W)
+ * with U_p = ceil(bytes_p / 16).  Each runs b200_allgather's staged protocol on the staging slots
+ * and launch counter shared by every collective, so it interleaves with them in stream order; a
+ * rank whose part is exhausted or empty still makes every launch.  A count list that differs
+ * between ranks breaks the contract, as mismatched send / recv sizes do; it cannot be detected
+ * locally.  Refused calls (NULL arrays, a NULL pointer with a non-zero count) launch nothing and
+ * return B200_ERR_INVALID; a bad dtype returns B200_ERR_UNSUPPORTED.  Replaces ProcessGroupNCCL's
+ * all-gather of unequal sizes, a coalesced group of one ncclBroadcast per rank. */
+int b200_allgatherv(b200_comm_t comm, const void *in, const size_t *counts, void *const *outs,
+                    int dtype, void *stream);
+
+/* Reduce-scatter with a size per rank.  counts: host array of world_size element counts, the same
+ * on every rank.  ins[q] (counts[q] elements) is this rank's contribution to rank q; out
+ * (counts[this rank] elements) = op over ranks of that rank's ins[this rank], rank-ascending, so
+ * it is bit-identical to b200_reducescatter on equal sizes.  A zero count moves nothing, and its
+ * pointer may be NULL; if all counts are zero nothing is launched.  When all counts are equal the
+ * call is exactly b200_reducescatter: it delegates, so it makes the same launches.  The only
+ * overlap allowed is the in-place form, out == ins[this rank].  World size 1: cudaMemcpyAsync when
+ * not in place, no kernel (AVG over one rank is the identity).  Launches: the output parts are cut
+ * into windows of W = floor(staging_bytes / (16 * world_size)) units, window w covering units
+ * [w * W, (w + 1) * W) of every part, so launches = ceil(max_q U_q / W) with U_q = ceil(bytes_q /
+ * 16); the world_size sub-slots of a window fill at most one staging slot.  Each runs on the
+ * staging slots and launch counter shared by every collective, so it interleaves with them in
+ * stream order.  A count list that differs between ranks breaks the contract, as mismatched send /
+ * recv sizes do; it cannot be detected locally.  Refused calls (NULL arrays, a NULL pointer with a
+ * non-zero count) launch nothing and return B200_ERR_INVALID; a bad dtype or op returns
+ * B200_ERR_UNSUPPORTED.  Replaces ProcessGroupNCCL's reduce-scatter of unequal sizes, a coalesced
+ * group of one ncclReduce per rank. */
+int b200_reducescatterv(b200_comm_t comm, const void *const *ins, const size_t *counts, void *out,
+                        int dtype, int op, void *stream);
+
 /* In-place copy of root's buffer to every rank.  Replaces ncclBroadcast at
  * nccl_collective_group.py:257-281. */
 int b200_broadcast(b200_comm_t comm, void *buf, size_t count, int dtype, int root,

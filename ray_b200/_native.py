@@ -85,6 +85,9 @@ SIGNATURES = {
     "b200_allreduce": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
     "b200_allgather": (c_int, [c_void_p, c_void_p, POINTER(c_void_p), c_size_t, c_int, c_void_p]),
     "b200_reducescatter": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_size_t, c_int, c_int, c_void_p]),
+    "b200_allgatherv": (c_int, [c_void_p, c_void_p, POINTER(c_size_t), POINTER(c_void_p), c_int, c_void_p]),
+    "b200_reducescatterv": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_size_t), c_void_p, c_int, c_int,
+                                    c_void_p]),
     "b200_broadcast": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
     "b200_reduce": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
     "b200_barrier": (c_int, [c_void_p, c_void_p]),

@@ -7,6 +7,7 @@ from .collective import (
     GroupManager,
     allgather,
     allgather_multi,
+    allgatherv,
     allreduce,
     barrier,
     broadcast,
@@ -22,6 +23,7 @@ from .collective import (
     reduce,
     reducescatter,
     reducescatter_multi,
+    reducescatterv,
     send,
     set_member_id,
     synchronize,
@@ -38,5 +40,6 @@ __all__ = [
     "register_collective_backend", "init_collective_group", "create_collective_group",
     "destroy_collective_group", "is_group_initialized", "get_rank", "get_collective_group_size",
     "get_group_handle", "allreduce", "barrier", "reduce", "broadcast", "broadcast_multi", "allgather", "allgather_multi",
-    "reducescatter", "reducescatter_multi", "send", "recv", "synchronize", "set_member_id", "use_manager",
+    "allgatherv", "reducescatter", "reducescatter_multi", "reducescatterv", "send", "recv", "synchronize",
+    "set_member_id", "use_manager",
 ]

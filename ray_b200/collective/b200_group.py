@@ -174,6 +174,30 @@ class B200Group(BaseGroup):
         _check_same_shape_dtype(out, ins)
         self._live().reducescatter(out, ins, _op_code(reducescatter_options.reduceOp))
 
+    def allgatherv(self, tensor_list, tensor):
+        """Extension beyond the reference API, whose ``allgather`` requires equal shapes:
+        ``tensor_list[p]`` receives rank p's ``tensor``, whose size may differ per rank.  Every rank
+        passes outputs of the same sizes; ``tensor_list[this rank]`` has this rank's size."""
+        if not isinstance(tensor_list, list):
+            raise RuntimeError("The output must be a list of tensors. Got '{}'.".format(type(tensor_list)))
+        t = _as_cuda_tensor(tensor)
+        outs = [_as_cuda_tensor(o) for o in tensor_list]
+        if len(outs) != self._world_size:
+            raise RuntimeError("The length of the tensor list operands to allgather must be equal to world_size.")
+        self._live().allgatherv(outs, t)
+
+    def reducescatterv(self, tensor, tensor_list, op=ReduceOp.SUM):
+        """Extension beyond the reference API, whose ``reducescatter`` requires equal shapes:
+        ``tensor`` = op over ranks of that rank's ``tensor_list[this rank]``; ``tensor_list[q]`` has
+        rank q's output size, the same on every rank."""
+        if not isinstance(tensor_list, list):
+            raise RuntimeError("The input must be a list of tensors. Got '{}'.".format(type(tensor_list)))
+        out = _as_cuda_tensor(tensor)
+        ins = [_as_cuda_tensor(i) for i in tensor_list]
+        if len(ins) != self._world_size:
+            raise RuntimeError("The length of the tensor list operands to reducescatter must be equal to world_size.")
+        self._live().reducescatterv(out, ins, _op_code(op))
+
     def allgather_multi(self, tensor_lists, tensors):
         """Extension beyond the reference API: ``allgather`` of a whole list of tensors (any dtypes)
         -- ``tensor_lists[i][p]`` receives rank p's ``tensors[i]`` -- in one launch per staging slot

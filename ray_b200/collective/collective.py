@@ -283,6 +283,39 @@ def reducescatter(tensor, tensor_list: list, group_name: str = "default", op=typ
     g.reducescatter([tensor], [tensor_list], opts)
 
 
+def allgatherv(tensor_list: list, tensor, group_name: str = "default") -> None:
+    """``allgather`` with a size per rank: ``tensor_list[p]`` receives rank p's ``tensor``.  An
+    extension beyond ``ray.util.collective``, whose ``allgather`` requires equal shapes, for
+    variable-length results (eval outputs, per-rank token counts, a sharded buffer whose last rank
+    holds the remainder).  Every rank passes outputs of the same sizes; the group's backend must
+    provide ``allgatherv`` (``B200Group`` does)."""
+    _check_single_tensor_input(tensor)
+    _check_tensor_list_input(tensor_list)
+    g = get_group_handle(group_name)
+    if len(tensor_list) != g.world_size:
+        raise RuntimeError("The length of the tensor list operands to allgather must be equal to world_size.")
+    if not hasattr(g, "allgatherv"):
+        raise RuntimeError("The collective group '{}' ({}) has no uneven all-gather.".format(
+            group_name, type(g).__name__))
+    g.allgatherv(tensor_list, tensor)
+
+
+def reducescatterv(tensor, tensor_list: list, group_name: str = "default", op=types.ReduceOp.SUM) -> None:
+    """``reducescatter`` with a size per rank: ``tensor`` = op over ranks of that rank's
+    ``tensor_list[this rank]``, where ``tensor_list[q]`` has rank q's output size on every rank.  The
+    mirror image of ``allgatherv``; the group's backend must provide ``reducescatterv``
+    (``B200Group`` does)."""
+    _check_single_tensor_input(tensor)
+    _check_tensor_list_input(tensor_list)
+    g = get_group_handle(group_name)
+    if len(tensor_list) != g.world_size:
+        raise RuntimeError("The length of the tensor list operands to reducescatter must be equal to world_size.")
+    if not hasattr(g, "reducescatterv"):
+        raise RuntimeError("The collective group '{}' ({}) has no uneven reduce-scatter.".format(
+            group_name, type(g).__name__))
+    g.reducescatterv(tensor, tensor_list, op)
+
+
 def _check_list_of_lists(tensor_lists, tensors, world_size: int, what: str) -> None:
     if not isinstance(tensor_lists, list):
         raise RuntimeError("The input must be a list of tensor lists. Got '{}'.".format(type(tensor_lists)))

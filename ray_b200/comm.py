@@ -293,6 +293,43 @@ class B200Comm:
         N.check(self._lib.b200_reducescatter(self._h, arr, out.data_ptr(), out.numel(),
                                              dtype_code(out.dtype), int(op), self._stream()))
 
+    def _uneven_parts(self, parts: Sequence[torch.Tensor], own: torch.Tensor, what: str, own_what: str):
+        """(pointer array, count array) of the world_size parts of an uneven all-gather or
+        reduce-scatter; the counts are the parts' numels and must match ``own`` at this rank."""
+        if len(parts) != self.world_size:
+            raise RuntimeError(f"The length of the tensor list operands to {what} must be equal to world_size.")
+        ptrs, counts = (ctypes.c_void_p * N.MAX_RANKS)(), (ctypes.c_size_t * N.MAX_RANKS)()
+        for p, t in enumerate(parts):
+            _check_cuda_contiguous(t, f"tensor {p}")
+            if t.dtype != own.dtype:
+                raise RuntimeError(f"All tensor operands to {what} must have the same dtype.")
+            ptrs[p] = t.data_ptr()
+            counts[p] = t.numel()
+        if parts[self.rank].numel() != own.numel():
+            raise RuntimeError(f"{what}: tensor {self.rank} (this rank's part) has {parts[self.rank].numel()} "
+                               f"elements, the {own_what} {own.numel()}")
+        return ptrs, counts
+
+    def allgatherv(self, outs: Sequence[torch.Tensor], tensor: torch.Tensor) -> None:
+        """``allgather`` with a size per rank: ``outs[p]`` receives rank p's ``tensor``, whose size
+        may differ per rank.  Every rank passes outputs of the same sizes, and ``outs[this rank]``
+        has this rank's size (it may be ``tensor`` itself).  Equal sizes run ``allgather``'s
+        launches; otherwise one launch per window of staging_bytes / 16 units of the largest part."""
+        _check_cuda_contiguous(tensor)
+        ptrs, counts = self._uneven_parts(outs, tensor, "allgatherv", "input has")
+        N.check(self._lib.b200_allgatherv(self._h, tensor.data_ptr(), counts, ptrs, dtype_code(tensor.dtype),
+                                          self._stream()))
+
+    def reducescatterv(self, out: torch.Tensor, ins: Sequence[torch.Tensor], op: int = N.SUM) -> None:
+        """``reducescatter`` with a size per rank: ``out`` = op over ranks of that rank's
+        ``ins[this rank]``, reduced rank-ascending; ``ins[q]`` has rank q's output size, the same on
+        every rank, and ``ins[this rank]`` may be ``out`` itself.  Equal sizes run
+        ``reducescatter``'s launches."""
+        _check_cuda_contiguous(out, "output tensor")
+        ptrs, counts = self._uneven_parts(ins, out, "reducescatterv", "output has")
+        N.check(self._lib.b200_reducescatterv(self._h, ptrs, counts, out.data_ptr(), dtype_code(out.dtype),
+                                              int(op), self._stream()))
+
     def allgather_multi(self, out_lists: Sequence[Sequence[torch.Tensor]], tensors: Sequence[torch.Tensor]) -> None:
         """``allgather`` of a list of tensors (any dtypes): ``out_lists[i][p]`` receives rank p's
         ``tensors[i]``.  One launch per staging slot of packed data (per ``N.P2P_TABLE_MAX``

@@ -56,6 +56,66 @@ __global__ void __launch_bounds__(kThreads, 1) allgather_kernel(DevComm c, AGArg
   finish_launch(c);
 }
 
+// One window of b200_allgatherv: units [w * W, (w + 1) * W) of every rank's part, W = staging_bytes / 16.
+// in and outs[p] point at the window's first byte of their part; nbytes[p] is what of rank p's part
+// falls in the window (0 once it is exhausted or empty), units = the largest ceil(nbytes[p] / 16).
+struct AGVArgs {
+  const char *in;
+  char *outs[kMaxRanks];
+  size_t nbytes[kMaxRanks];
+  size_t units;
+  size_t staging_bytes;
+};
+
+// allgather_kernel's protocol with a size per rank.  The CTA barrier pairs CTA b of every rank, so
+// CTA b must handle the same unit indices on every rank in both phases: the grid (pick_blocks on
+// the window's largest part), the unit -> CTA mapping (grid-stride over [0, units)) and the number
+// of launches are functions of the size list, staging_bytes and the grid cap alone, never of this
+// rank's own size or alignment.  A unit past a rank's part is skipped, and a rank whose part is
+// exhausted still launches and crosses the barrier (DESIGN.md §3: every rank makes every launch).
+__global__ void __launch_bounds__(kThreads, 1) allgatherv_kernel(DevComm c, AGVArgs a) {
+  const uint32_t launch = c.st->launch_ctr;
+  const uint32_t ep = launch * 4u;
+  const int n = c.world, r = c.rank;
+  const size_t U = a.units;
+  const size_t off = staging_slot_offset(launch, a.staging_bytes);
+  const size_t stride = size_t(gridDim.x) * kThreads;
+  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
+
+  const Units mine_un = make_units(a.nbytes[r]);
+  const size_t mine_U = mine_un.total();
+  const bool in_al = is_aligned16(a.in);
+  char *mine = c.data[r] + off;
+  for (size_t u = first; u < mine_U; u += stride) st_vec(mine + (u << 4), load_user_unit(a.in, u, mine_un, in_al));
+
+  if (!cta_barrier_all(c, ep + 1)) {
+    finish_launch(c);
+    return;
+  }
+
+  for (size_t u = first; u < U; u += stride) {
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int p = r + i;
+        if (p >= n) p -= n;
+        if (u < make_units(a.nbytes[p]).total()) v[i] = ld_peer(c.data[p] + off + (u << 4));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int p = r + i;
+        if (p >= n) p -= n;
+        const Units un = make_units(a.nbytes[p]);
+        if (u < un.total()) store_user_unit(a.outs[p], u, un, is_aligned16(a.outs[p]), v[i]);
+      }
+    }
+  }
+  finish_launch(c);
+}
+
 struct BcastArgs {
   char *buf;
   size_t nbytes;
@@ -251,6 +311,41 @@ extern "C" int b200_allgather(b200_comm_t c, const void *in, void *const *outs, 
     const size_t U = make_units(nbytes).total();
     int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
     allgather_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
+    B200_LAUNCH_CHECK(c);
+    return B200_OK;
+  });
+}
+
+extern "C" int b200_allgatherv(b200_comm_t c, const void *in, const size_t *counts, void *const *outs, int dtype,
+                               void *stream_) {
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_list(c->world, counts && outs)))
+    return rc;
+  const int n = c->world;
+  size_t nbytes[kMaxRanks] = {};
+  bool even = true;
+  for (int p = 0; p < n; ++p) {
+    nbytes[p] = counts[p] * es;
+    even = even && counts[p] == counts[0];
+  }
+  if ((rc = check_list_ptrs(outs, nbytes, n))) return rc;
+  if (nbytes[c->rank] && !in) return null_tensor_error();
+  if (even) return b200_allgather(c, in, outs, counts[0], dtype, stream_);  // also world 1
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  AGVArgs a{};
+  a.staging_bytes = c->staging_bytes;
+  const VPlan plan = v_plan(nbytes, n, c->staging_bytes / 16);
+  return for_each_piece(plan.max_units, plan.window_units, [&](size_t u0, size_t units) -> int {
+    for (int p = 0; p < n; ++p) {
+      a.nbytes[p] = v_window_bytes(nbytes[p], u0, units);
+      a.outs[p] = a.nbytes[p] ? static_cast<char *>(outs[p]) + (u0 << 4) : nullptr;
+    }
+    a.in = a.nbytes[c->rank] ? static_cast<const char *>(in) + (u0 << 4) : nullptr;
+    a.units = units;
+    int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+    allgatherv_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
     B200_LAUNCH_CHECK(c);
     return B200_OK;
   });

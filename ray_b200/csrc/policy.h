@@ -155,6 +155,31 @@ inline bool ag_pull_pays_off(const b200_comm *c, size_t nbytes) {
   return nbytes >= (v > 0 ? size_t(v) : (size_t(4) << 20));
 }
 
+// Windows of the uneven all-gather and reduce-scatter (b200_allgatherv, b200_reducescatterv): window
+// w covers units [w * W, (w + 1) * W) of every rank's part, so launches = ceil(max_units / W).  The
+// plan is a function of the size list and W (from staging_bytes and the world size) alone, so every
+// rank makes the same launches whatever its own part.
+struct VPlan {
+  size_t max_units;     // the largest part, in 16-byte units
+  size_t window_units;  // W
+};
+inline VPlan v_plan(const size_t *nbytes, int n, size_t window_units) {
+  VPlan v{0, window_units};
+  for (int p = 0; p < n; ++p) {
+    const size_t u = (nbytes[p] + 15) / 16;
+    if (u > v.max_units) v.max_units = u;
+  }
+  return v;
+}
+// Bytes of a part of `nbytes` inside the window of `units` units that starts at unit u0 (0 once the
+// part is exhausted).
+inline size_t v_window_bytes(size_t nbytes, size_t u0, size_t units) {
+  const size_t done = u0 << 4;
+  if (nbytes <= done) return 0;
+  const size_t left = nbytes - done;
+  return left < (units << 4) ? left : (units << 4);
+}
+
 // The multicast store pays off once more than one peer would pull from the root.
 inline bool broadcast_nvls(const b200_comm *c, size_t nbytes) {
   return c->mc_active && c->world > 2 && nbytes >= (size_t(64) << 10);

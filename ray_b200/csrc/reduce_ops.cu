@@ -71,6 +71,77 @@ __global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, R
   finish_launch(c);
 }
 
+// One window of b200_reducescatterv: units [w * W, (w + 1) * W) of every rank's output part,
+// W = floor(staging_bytes / (16 * n)).  ins[q] and out point at the window's first byte of their
+// part; nbytes[q] is what of rank q's part falls in the window (0 once it is exhausted or empty).
+// units = the largest ceil(nbytes[q] / 16): every sub-slot is units * 16 bytes, so the n sub-slots
+// fit one staging slot and both sides derive the layout from the shared sizes.
+struct RSVArgs {
+  const char *ins[kMaxRanks];
+  char *out;
+  size_t nbytes[kMaxRanks];
+  size_t units;
+  size_t staging_bytes;
+};
+
+// reducescatter_kernel's push with a size per rank: rank r pushes the window's units of ins[q] into
+// sub-slot r of rank q's slot, crosses the barrier, then reduces its own n sub-slots rank-ascending
+// over its own part's units.  The CTA barrier pairs CTA b of every rank, so the grid (pick_blocks
+// on the window's largest part), the unit -> CTA mapping (grid-stride over [0, units)) and the
+// number of launches depend only on the size list, staging_bytes and the grid cap -- never on this
+// rank's own size or alignment.  A rank whose part is exhausted still launches and crosses the
+// barrier (DESIGN.md §3).  Every output element has n contributions, so AVG divides by n.
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reducescatterv_kernel(DevComm c, RSVArgs a) {
+  const uint32_t launch = c.st->launch_ctr;
+  const uint32_t ep = launch * 4u;
+  const int n = c.world, r = c.rank;
+  const size_t U = a.units;
+  const size_t sub = U << 4;  // bytes per sub-slot
+  const size_t off = staging_slot_offset(launch, a.staging_bytes);
+  const size_t stride = size_t(gridDim.x) * kThreads;
+  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
+
+  for (size_t u = first; u < U; u += stride) {
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int q = r + i;
+        if (q >= n) q -= n;
+        const Units un = make_units(a.nbytes[q]);
+        if (u < un.total()) v[i] = load_user_unit(a.ins[q], u, un, is_aligned16(a.ins[q]));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kMaxRanks; ++i) {
+      if (i < n) {
+        int q = r + i;
+        if (q >= n) q -= n;
+        if (u < make_units(a.nbytes[q]).total()) st_vec(c.data[q] + off + size_t(r) * sub + (u << 4), v[i]);
+      }
+    }
+  }
+
+  if (!cta_barrier_all(c, ep + 1)) {
+    finish_launch(c);
+    return;
+  }
+
+  const Units un = make_units(a.nbytes[r]);
+  const size_t mine_U = un.total();
+  const bool out_al = is_aligned16(a.out);
+  const char *mine = c.data[r] + off;
+  for (size_t u = first; u < mine_U; u += stride) {
+    uint4 v[kMaxRanks];
+#pragma unroll
+    for (int p = 0; p < kMaxRanks; ++p)
+      if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
+    store_user_unit(a.out, u, un, out_al, reduce_ranks<T, OP>(v, n));
+  }
+  finish_launch(c);
+}
+
 // One window [u0, u0 + units) of a table's packed stream of output units; n sub-slots of
 // units * 16 bytes fit one staging slot.
 struct RSTableArgs {
@@ -230,6 +301,45 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
     int rc2 = B200_OK;
     B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc2 = launch_rs<T, OP>(c, a, stream); }));
     return rc2;
+  });
+}
+
+extern "C" int b200_reducescatterv(b200_comm_t c, const void *const *ins, const size_t *counts, void *out,
+                                   int dtype, int op, void *stream_) {
+  int rc;
+  size_t es;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op)) ||
+      (rc = check_list(c->world, ins && counts)))
+    return rc;
+  const int n = c->world;
+  size_t nbytes[kMaxRanks] = {};
+  bool even = true;
+  for (int q = 0; q < n; ++q) {
+    nbytes[q] = counts[q] * es;
+    even = even && counts[q] == counts[0];
+  }
+  if ((rc = check_list_ptrs(const_cast<void *const *>(ins), nbytes, n))) return rc;
+  if (nbytes[c->rank] && !out) return null_tensor_error();
+  if (even) return b200_reducescatter(c, ins, out, counts[0], dtype, op, stream_);  // also world 1
+  void (*kernel)(DevComm, RSVArgs) = nullptr;
+  B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatterv_kernel<T, OP>; }));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  RSVArgs a{};
+  a.staging_bytes = c->staging_bytes;
+  // the n sub-slots of a window fill at most one staging slot
+  const VPlan plan = v_plan(nbytes, n, c->staging_bytes / (16 * size_t(n)));
+  return for_each_piece(plan.max_units, plan.window_units, [&](size_t u0, size_t units) -> int {
+    for (int q = 0; q < n; ++q) {
+      a.nbytes[q] = v_window_bytes(nbytes[q], u0, units);
+      a.ins[q] = a.nbytes[q] ? static_cast<const char *>(ins[q]) + (u0 << 4) : nullptr;
+    }
+    a.out = a.nbytes[c->rank] ? static_cast<char *>(out) + (u0 << 4) : nullptr;
+    a.units = units;
+    int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+    kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
+    B200_LAUNCH_CHECK(c);
+    return B200_OK;
   });
 }
 

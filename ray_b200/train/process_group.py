@@ -320,9 +320,19 @@ class B200ProcessGroup(dist.ProcessGroup):
             ins.append(i)
         return list(groups.values())
 
+    @staticmethod
+    def _refuse_uneven_lists(what: str, pairs) -> None:
+        """The list forms have no uneven variant: every (tensor, per-rank tensors) pair must agree in
+        size.  One tensor of uneven parts goes through all_gather / reduce_scatter instead."""
+        for i, (t, per_rank) in enumerate(pairs):
+            if any(x.numel() != t.numel() for x in per_rank):
+                raise RuntimeError(f"b200 process group: {what} of a tensor list needs equal sizes on every rank "
+                                   f"(tensor {i} differs); uneven sizes are supported for a single tensor only")
+
     def _allgather_lists(self, output_lists, inputs) -> B200Work:
         """output_lists[i][p] receives rank p's inputs[i], in one b200_allgather_multi call; an output
         list that is not contiguous receives through temporaries and a copy."""
+        self._refuse_uneven_lists("all_gather", zip(inputs, output_lists))
 
         def fn(comm):
             lists = [list(outs) if all(o.is_contiguous() for o in outs) else [torch.empty_like(t) for _ in outs]
@@ -344,8 +354,19 @@ class B200ProcessGroup(dist.ProcessGroup):
 
         def fn(comm):
             for outs, t in zip(output_tensors, input_tensors):
+                # parts of a different size per rank: one b200_allgatherv call where ProcessGroupNCCL
+                # falls back to a coalesced broadcast per rank
+                uneven = any(o.numel() != t.numel() for o in outs)
                 if all(o.is_contiguous() for o in outs):
-                    comm.allgather(list(outs), self._contig(t))
+                    if uneven:
+                        comm.allgatherv(list(outs), self._contig(t))
+                    else:
+                        comm.allgather(list(outs), self._contig(t))
+                elif uneven:
+                    tmp = [torch.empty(o.shape, dtype=o.dtype, device=o.device) for o in outs]
+                    comm.allgatherv(tmp, self._contig(t))
+                    for o, s in zip(outs, tmp):
+                        o.copy_(s)
                 else:
                     tmp = [torch.empty_like(t) for _ in outs]
                     comm.allgather(tmp, self._contig(t))
@@ -386,6 +407,8 @@ class B200ProcessGroup(dist.ProcessGroup):
             return self._cpu_group().reduce_scatter(output_tensors, input_tensors, opts)
         op = _op_code(opts.reduceOp) if opts is not None else N.SUM
         if len(output_tensors) > 1:
+            self._refuse_uneven_lists("reduce_scatter", zip(output_tensors, input_tensors))
+
             def fn_multi(comm):
                 for outs, ins in self._by_dtype(output_tensors, input_tensors):
                     comm.reducescatter_multi([self._contig(o) for o in outs],
@@ -396,7 +419,12 @@ class B200ProcessGroup(dist.ProcessGroup):
 
         def fn(comm):
             for out, ins in zip(output_tensors, input_tensors):
-                comm.reducescatter(self._contig(out), [self._contig(i) for i in ins], op)
+                # parts of a different size per rank: one b200_reducescatterv call where
+                # ProcessGroupNCCL falls back to a coalesced reduce per rank
+                if any(i.numel() != out.numel() for i in ins):
+                    comm.reducescatterv(self._contig(out), [self._contig(i) for i in ins], op)
+                else:
+                    comm.reducescatter(self._contig(out), [self._contig(i) for i in ins], op)
 
         flat = list(output_tensors) + [i for ins in input_tensors for i in ins]
         return self._run(flat, fn, output_tensors)

@@ -6,9 +6,10 @@ GPU, launches replayed from CUDA graphs so host launch overhead does not pollute
                                             grad_rs|grad_rs_unfused|alltoall|alltoall_p2p|
                                             sendrecv_multi|sendrecv_loop|bcast_multi|bcast_loop|
                                             bcast_coalesced|ag_multi|ag_loop|ag_flat|rs_multi|rs_loop|rs_flat|
-                                            exchange_batch|exchange_ordered|ring_batch|ring_ordered]
+                                            exchange_batch|exchange_ordered|ring_batch|ring_ordered|
+                                            agv|agv_pad|agv_a2a|rsv|rsv_pad|rsv_reduce]
         [--tensors 16,256,resnet50,resnet50_buffers]
-        [--split uniform|skew|local] [--wire bfloat16]
+        [--split uniform|skew|local|ragged|one_empty] [--wire bfloat16]
 
 Prints one line per (size, algo, blocks): us per launch, algbw, busbw (nccl-tests convention).
 --op takes a comma list; the ops then alternate at every size.  For the gradient reduce-scatter
@@ -32,6 +33,14 @@ b200_allgather, one multi-tensor copy back into the outputs.  ``rs_multi``, ``rs
 rank's part, so every rank holds world_size times it.
 The list comes from --tensors: N equal tensors of size / N bytes, ResNet-50's parameter list or
 ResNet-50's buffers (fp32 and int64).
+``agv`` all-gathers parts of a different size per rank with b200_allgatherv, ``agv_pad`` pads every
+part to the largest and runs b200_allgather (the outputs are views of the padded result), ``agv_a2a``
+sends the part to every peer with one b200_alltoall.  ``rsv`` reduce-scatters uneven parts with
+b200_reducescatterv, ``rsv_pad`` copies the inputs into padded parts and runs b200_reducescatter, and
+``rsv_reduce`` makes one b200_reduce per root, as ProcessGroupNCCL does.  Their parts come from
+--split: uniform (`size` bytes each), ragged (a few elements off `size`, the last rank a third
+shorter), skew (size >> r on rank r) or one_empty (the last rank's part is empty).  Their algbw
+counts the sum of all parts.
 ``exchange_batch`` is a two-rank bidirectional exchange of `size` bytes per direction, both directions
 as one b200_p2p_batch per rank; ``exchange_ordered`` is the same exchange as plain send / recv in an
 order that cannot wait on itself (even ranks send first, odd ranks receive first).  ``ring_batch`` and
@@ -200,6 +209,73 @@ def rs_flat(c, n, outs, ins, flat_in, flat_out):
     torch._foreach_copy_(outs, list(flat_out.split([o.numel() for o in outs])))
 
 
+V_OPS = ("agv", "agv_pad", "agv_a2a", "rsv", "rsv_pad", "rsv_reduce")
+
+
+def v_counts(n, numel, split):
+    """Element count of every rank's part for the uneven all-gather / reduce-scatter ops."""
+    if split == "ragged":  # a few elements off `size`, the last rank shorter (a sharded buffer's remainder)
+        return [numel + (p % 3) - 1 for p in range(n - 1)] + [numel - numel // 3]
+    if split == "skew":  # 4:2:1...
+        return [max(numel >> p, 1) for p in range(n)]
+    if split == "one_empty":
+        return [numel] * (n - 1) + [0]
+    if split == "uniform":
+        return [numel] * n
+    raise SystemExit(f"--split {split} does not apply to the uneven all-gather / reduce-scatter ops")
+
+
+def v_call(g, n, op, counts, dtype):
+    """The launch sequence of one uneven op on rank r, as call(c, r), and the bytes one rank gathers
+    (all-gather) or reduces (reduce-scatter) in total.
+      agv        b200_allgatherv
+      agv_pad    copy the part into a buffer padded to the largest part, b200_allgather, use views
+      agv_a2a    b200_alltoall with the part sent to every peer (the one-launch route without agv)
+      rsv        b200_reducescatterv
+      rsv_pad    copy the n inputs into padded parts, b200_reducescatter, use a view of the output
+      rsv_reduce one b200_reduce per root (ProcessGroupNCCL's uneven reduce-scatter)"""
+    m = max(counts)
+    dev = g.device
+    mine = [torch.ones(counts[r], dtype=dtype, device=dev(r)) for r in range(n)]
+    if op == "agv":
+        outs = [[torch.empty(k, dtype=dtype, device=dev(r)) for k in counts] for r in range(n)]
+        call = lambda c, r: c.allgatherv(outs[r], mine[r])  # noqa: E731
+    elif op == "agv_pad":
+        pad_in = [torch.zeros(m, dtype=dtype, device=dev(r)) for r in range(n)]
+        pad_out = [torch.empty(n * m, dtype=dtype, device=dev(r)) for r in range(n)]
+
+        def call(c, r):
+            pad_in[r][:counts[r]].copy_(mine[r])
+            c.allgather_into(pad_out[r], pad_in[r])
+    elif op == "agv_a2a":
+        outs = [[torch.empty(k, dtype=dtype, device=dev(r)) for k in counts] for r in range(n)]
+        call = lambda c, r: c.alltoall(outs[r], [mine[r]] * n)  # noqa: E731
+    else:
+        ins = [[torch.ones(k, dtype=dtype, device=dev(r)) for k in counts] for r in range(n)]
+        if op == "rsv":
+            call = lambda c, r: c.reducescatterv(mine[r], ins[r], N.SUM)  # noqa: E731
+        elif op == "rsv_pad":
+            pad_in = [torch.zeros(n, m, dtype=dtype, device=dev(r)) for r in range(n)]
+            pad_out = [torch.empty(m, dtype=dtype, device=dev(r)) for r in range(n)]
+
+            def call(c, r):
+                torch._foreach_copy_([pad_in[r][q, :counts[q]] for q in range(n)], ins[r])
+                c.reducescatter_from(pad_out[r], pad_in[r].view(-1), N.SUM)
+        elif op == "rsv_reduce":
+            call = lambda c, r: [c.reduce(ins[r][q], q, N.SUM) for q in range(n)]  # noqa: E731
+        else:
+            raise SystemExit(f"unknown op {op}")
+    # load the torch copy kernels outside any collective (see the grad_rs_unfused branch of main)
+    for r in range(n):
+        with torch.cuda.device(g.devices[r]):
+            if op == "agv_pad":
+                pad_in[r][:counts[r]].copy_(mine[r])
+            elif op == "rsv_pad":
+                torch._foreach_copy_([pad_in[r][q, :counts[q]] for q in range(n)], ins[r])
+    es = torch.empty((), dtype=dtype).element_size()
+    return call, sum(counts) * es
+
+
 def grad_rs_unfused(c, out, grad, wout, scale, wire):
     """The composition the fused gradient reduce-scatter replaces: scale, cast to the wire type,
     reduce-scatter in the wire type, cast the shard back into the fp32 output."""
@@ -220,8 +296,8 @@ def main():
     ap.add_argument("--symm", action="store_true", help="operands in the symmetric heap (zero copy)")
     ap.add_argument("--nvls-min-world", type=int, default=-1)
     ap.add_argument("--nvls-ctas", default="-1", help="comma list of CTA counts for the NVLS reduce phase")
-    ap.add_argument("--split", default="uniform", choices=["uniform", "skew", "local"],
-                    help="all-to-all ops: bytes per peer (see above)")
+    ap.add_argument("--split", default="uniform", choices=["uniform", "skew", "local", "ragged", "one_empty"],
+                    help="all-to-all ops: bytes per peer; agv / rsv ops: part per rank (see above)")
     ap.add_argument("--wire", default="bfloat16", help="wire dtype of the grad_rs ops")
     ap.add_argument("--tensors", default="1",
                     help="list ops: comma list of recipes, N (N equal tensors of size / N bytes), "
@@ -312,6 +388,9 @@ def main():
                         else:
                             call = lambda c, r: alltoall_p2p(c, r, n, outs[r], ins[r], side[r])  # noqa: E731
                         factor = (n - 1) / n  # nccl-tests all-to-all: busbw = algbw * (n-1)/n
+                    elif op in V_OPS:
+                        call, nbytes = v_call(g, n, op, v_counts(n, numel, args.split), dtype)
+                        factor = (n - 1) / n  # of the bytes gathered / reduced per rank
                     elif op in ("exchange_batch", "exchange_ordered", "ring_batch", "ring_ordered"):
                         k = n if op.startswith("ring") else 2
                         if k < 3 and op.startswith("ring"):
@@ -324,7 +403,7 @@ def main():
                         raise SystemExit(f"unknown op {op}")
                     torch.cuda.synchronize()
                     us = time_graphs(g, call, iters)
-                    algbw = (nbytes if op.startswith("alltoall") else size) / us / 1e3
+                    algbw = (nbytes if op.startswith("alltoall") or op in V_OPS else size) / us / 1e3
                     print(f"{op} {size:>11d} B  algo={aname:8s} blocks={blocks:3d} nvls_ctas={nctas:3d} {us:10.2f} us  "
                           f"algbw={algbw:8.1f} GB/s  busbw={algbw * factor:8.1f} GB/s", flush=True)
                     del xs
