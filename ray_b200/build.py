@@ -24,7 +24,7 @@ LIB_PATH = PKG_DIR / "libb200_collective.so"
 
 SOURCES = ["bootstrap.cu", "allreduce.cu", "allreduce_pipe.cu", "reduce_ops.cu", "copy_ops.cu", "p2p.cu", "grad.cu"]
 HEADERS = ["common.cuh", "comm.h", "kernel_utils.cuh", "allreduce_core.cuh", "bulk_copy.cuh", "pipe.h", "policy.h",
-           "tensor_table.cuh"]
+           "staged.cuh", "tensor_table.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -20,6 +20,7 @@
 // no grid-wide sync, no host involvement.
 #include "allreduce_core.cuh"
 #include "policy.h"
+#include "tensor_table.cuh"
 
 namespace b200 {
 
@@ -196,7 +197,7 @@ allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t
   const size_t off = staging_slot_offset(launch, staging_bytes);
 
   stage_in_rows(c, off, g, [&](size_t u) {
-    const int i = table_find(tb, u);
+    const int i = table_entry(tb.ustart, tb.count, u);
     return load_user_unit(tb.ptr[i], u - tb.ustart[i], make_units(tb.nbytes[i]), is_aligned16(tb.ptr[i]));
   });
   if (!reduce_phase<T, OP, NVLS>(c, ep, off, g, red_ctas)) {
@@ -204,7 +205,7 @@ allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t
     return;
   }
   stage_out_rows(c, off, g, [&](size_t u, uint4 v) {
-    const int i = table_find(tb, u);
+    const int i = table_entry(tb.ustart, tb.count, u);
     store_user_unit(tb.ptr[i], u - tb.ustart[i], make_units(tb.nbytes[i]), is_aligned16(tb.ptr[i]), v);
   });
   finish_launch(c);

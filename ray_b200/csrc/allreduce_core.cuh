@@ -177,14 +177,4 @@ struct TensorTable {
   unsigned int ustart[kMaxTableTensors + 1];
 };
 
-__device__ __forceinline__ int table_find(const TensorTable &tb, size_t u) {
-  int lo = 0, hi = tb.count - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (tb.ustart[mid] <= u) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
-}
-
 }  // namespace b200

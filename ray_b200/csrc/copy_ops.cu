@@ -1,7 +1,9 @@
 // copy_ops.cu — all-gather (SURVEY K2 with the K6 un-flatten copies fused away) and
 // broadcast (K4), each of one tensor or of a tensor list, and the flag-only barrier (K7).
-// These kernels move bytes; they do not depend on the element type.
+// These kernels move bytes; they do not depend on the element type.  The staged protocols of
+// both collectives live in staged.cuh; each kernel here says where a unit comes from and goes.
 #include "policy.h"
+#include "staged.cuh"
 #include "tensor_table.cuh"
 
 namespace b200 {
@@ -13,47 +15,12 @@ struct AGArgs {
   size_t staging_bytes;
 };
 
-// Every rank stages its tensor in its own slot, then pulls each peer's slot over
-// NVLink straight into the caller's output tensor for that peer.
 __global__ void __launch_bounds__(kThreads, 1) allgather_kernel(DevComm c, AGArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int n = c.world, r = c.rank;
   const Units un = make_units(a.nbytes);
-  const size_t U = un.total();
   const bool in_al = is_aligned16(a.in);
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), load_user_unit(a.in, u, un, in_al));
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  for (size_t u = first; u < U; u += stride) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int p = r + i;
-        if (p >= n) p -= n;
-        v[i] = ld_peer(c.data[p] + off + (u << 4));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int p = r + i;
-        if (p >= n) p -= n;
-        store_user_unit(a.outs[p], u, un, is_aligned16(a.outs[p]), v[i]);
-      }
-    }
-  }
-  finish_launch(c);
+  allgather_body(
+      c, a.staging_bytes, un.total(), un.total(), [&](size_t u) { return load_user_unit(a.in, u, un, in_al); },
+      [&](size_t u) { return PeerParts<char *>{a.outs, u, un}; });
 }
 
 // One window of b200_allgatherv: units [w * W, (w + 1) * W) of every rank's part, W = staging_bytes / 16.
@@ -67,53 +34,27 @@ struct AGVArgs {
   size_t staging_bytes;
 };
 
-// allgather_kernel's protocol with a size per rank.  The CTA barrier pairs CTA b of every rank, so
-// CTA b must handle the same unit indices on every rank in both phases: the grid (pick_blocks on
-// the window's largest part), the unit -> CTA mapping (grid-stride over [0, units)) and the number
-// of launches are functions of the size list, staging_bytes and the grid cap alone, never of this
-// rank's own size or alignment.  A unit past a rank's part is skipped, and a rank whose part is
-// exhausted still launches and crosses the barrier (DESIGN.md §3: every rank makes every launch).
+// Unit u of the uneven parts: rank p's part has it while u < ceil(nbytes[p] / 16).
+struct AGVUnit {
+  const AGVArgs &a;
+  size_t u;
+  __device__ __forceinline__ bool has(int p) const { return u < make_units(a.nbytes[p]).total(); }
+  __device__ __forceinline__ void store(int p, uint4 v) const {
+    const Units un = make_units(a.nbytes[p]);
+    if (u < un.total()) store_user_unit(a.outs[p], u, un, is_aligned16(a.outs[p]), v);
+  }
+};
+
+// The grid (pick_blocks on the window's largest part), the unit -> CTA mapping (grid-stride over
+// [0, units)) and the number of launches are functions of the size list, staging_bytes and the
+// grid cap alone, never of this rank's own size or alignment.  A rank whose part is exhausted
+// still launches and crosses the barrier (DESIGN.md §3: every rank makes every launch).
 __global__ void __launch_bounds__(kThreads, 1) allgatherv_kernel(DevComm c, AGVArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int n = c.world, r = c.rank;
-  const size_t U = a.units;
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  const Units mine_un = make_units(a.nbytes[r]);
-  const size_t mine_U = mine_un.total();
+  const Units mine_un = make_units(a.nbytes[c.rank]);
   const bool in_al = is_aligned16(a.in);
-  char *mine = c.data[r] + off;
-  for (size_t u = first; u < mine_U; u += stride) st_vec(mine + (u << 4), load_user_unit(a.in, u, mine_un, in_al));
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  for (size_t u = first; u < U; u += stride) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int p = r + i;
-        if (p >= n) p -= n;
-        if (u < make_units(a.nbytes[p]).total()) v[i] = ld_peer(c.data[p] + off + (u << 4));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int p = r + i;
-        if (p >= n) p -= n;
-        const Units un = make_units(a.nbytes[p]);
-        if (u < un.total()) store_user_unit(a.outs[p], u, un, is_aligned16(a.outs[p]), v[i]);
-      }
-    }
-  }
-  finish_launch(c);
+  allgather_body(
+      c, a.staging_bytes, mine_un.total(), a.units, [&](size_t u) { return load_user_unit(a.in, u, mine_un, in_al); },
+      [&](size_t u) { return AGVUnit{a, u}; });
 }
 
 struct BcastArgs {
@@ -123,40 +64,13 @@ struct BcastArgs {
   int root;
 };
 
-// NVLS = false: root stages, every other rank pulls root's slot.
-// NVLS = true : root writes its tensor once to the multicast alias (the switch
-//               replicates it into every rank's slot), the others copy out locally.
 template <bool NVLS>
 __global__ void __launch_bounds__(kThreads, 1) broadcast_kernel(DevComm c, BcastArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int r = c.rank;
   const Units un = make_units(a.nbytes);
-  const size_t U = un.total();
   const bool al = is_aligned16(a.buf);
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  if (r == a.root) {
-    char *dst = (NVLS ? c.mc_data : c.data[r]) + off;
-    for (size_t u = first; u < U; u += stride) {
-      const uint4 v = load_user_unit(a.buf, u, un, al);
-      if (NVLS) multimem_st(dst + (u << 4), v);
-      else st_vec(dst + (u << 4), v);
-    }
-  }
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  if (r != a.root) {
-    const char *src = (NVLS ? c.data[r] : c.data[a.root]) + off;
-    for (size_t u = first; u < U; u += stride) store_user_unit(a.buf, u, un, al, ld_peer(src + (u << 4)));
-  }
-  finish_launch(c);
+  broadcast_body<NVLS>(
+      c, a.staging_bytes, a.root, un.total(), [&](size_t u) { return load_user_unit(a.buf, u, un, al); },
+      [&](size_t u, uint4 v) { store_user_unit(a.buf, u, un, al, v); });
 }
 
 // One window of a table's packed stream (tensor_table.cuh): units [u0, u0 + units), at most one
@@ -169,38 +83,12 @@ struct BcastTableArgs {
   int root;
 };
 
-// broadcast_kernel's protocol for a window of a table (b200_broadcast_multi): unit u0 + u of the
-// stream goes through byte u * 16 of the staging slot.
 template <bool NVLS>
 __global__ void __launch_bounds__(kThreads, 1)
     broadcast_table_kernel(DevComm c, const __grid_constant__ BcastTableArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int r = c.rank;
-  const size_t U = a.units;
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  if (r == a.root) {
-    char *dst = (NVLS ? c.mc_data : c.data[r]) + off;
-    for (size_t u = first; u < U; u += stride) {
-      const uint4 v = table_load_unit(a.t, a.u0 + u);
-      if (NVLS) multimem_st(dst + (u << 4), v);
-      else st_vec(dst + (u << 4), v);
-    }
-  }
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  if (r != a.root) {
-    const char *src = (NVLS ? c.data[r] : c.data[a.root]) + off;
-    for (size_t u = first; u < U; u += stride) table_store_unit(a.t, a.u0 + u, ld_peer(src + (u << 4)));
-  }
-  finish_launch(c);
+  broadcast_body<NVLS>(
+      c, a.staging_bytes, a.root, a.units, [&](size_t u) { return table_load_unit(a.t, a.u0 + u); },
+      [&](size_t u, uint4 v) { table_store_unit(a.t, a.u0 + u, v); });
 }
 
 // One window [u0, u0 + units) of a table's packed stream of input units, at most one staging slot.
@@ -213,50 +101,14 @@ struct AGTableArgs {
 };
 static_assert(fits_param_space<AGTableArgs>(), "all-gather table exceeds the kernel parameter space");
 
-// allgather_kernel's protocol for a window of a table (b200_allgather_multi): every rank stages
-// unit u0 + u of its stream at byte u * 16 of its own slot, then pulls each peer's slot into
-// the owning entry's output for that peer.
 __global__ void __launch_bounds__(kThreads, 1)
     allgather_table_kernel(DevComm c, const __grid_constant__ AGTableArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int n = c.world, r = c.rank;
-  const size_t U = a.units;
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), table_load_unit(a.t, a.u0 + u));
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  for (size_t u = first; u < U; u += stride) {
-    const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
-    const size_t lu = a.u0 + u - a.t.ustart[k];
-    const Units un = make_units(a.t.nbytes[k]);
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int p = r + i;
-        if (p >= n) p -= n;
-        v[i] = ld_peer(c.data[p] + off + (u << 4));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int p = r + i;
-        if (p >= n) p -= n;
-        store_user_unit(a.outs[k][p], lu, un, is_aligned16(a.outs[k][p]), v[i]);
-      }
-    }
-  }
-  finish_launch(c);
+  allgather_body(
+      c, a.staging_bytes, a.units, a.units, [&](size_t u) { return table_load_unit(a.t, a.u0 + u); },
+      [&](size_t u) {
+        const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
+        return PeerParts<char *>{a.outs[k], a.u0 + u - a.t.ustart[k], make_units(a.t.nbytes[k])};
+      });
 }
 
 __global__ void barrier_kernel(DevComm c) {
@@ -308,11 +160,7 @@ extern "C" int b200_allgather(b200_comm_t c, const void *in, void *const *outs, 
     for (int p = 0; p < c->world; ++p) a.outs[p] = static_cast<char *>(outs[p]) + done;
     a.nbytes = nbytes;
     a.staging_bytes = c->staging_bytes;
-    const size_t U = make_units(nbytes).total();
-    int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
-    allgather_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
-    B200_LAUNCH_CHECK(c);
-    return B200_OK;
+    return launch_staged(c, allgather_kernel, a, make_units(nbytes).total(), stream);
   });
 }
 
@@ -344,10 +192,7 @@ extern "C" int b200_allgatherv(b200_comm_t c, const void *in, const size_t *coun
     }
     a.in = a.nbytes[c->rank] ? static_cast<const char *>(in) + (u0 << 4) : nullptr;
     a.units = units;
-    int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
-    allgatherv_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
-    B200_LAUNCH_CHECK(c);
-    return B200_OK;
+    return launch_staged(c, allgatherv_kernel, a, units, stream);
   });
 }
 
@@ -361,13 +206,9 @@ extern "C" int b200_broadcast(b200_comm_t c, void *buf, size_t count, int dtype,
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   return for_each_piece(count * es, c->staging_bytes, [&](size_t done, size_t nbytes) -> int {
-    BcastArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
-    const size_t U = make_units(nbytes).total();
-    int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
-    if (broadcast_nvls(c, nbytes)) broadcast_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
-    else broadcast_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
-    B200_LAUNCH_CHECK(c);
-    return B200_OK;
+    const BcastArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
+    return launch_staged(c, broadcast_nvls(c, nbytes) ? broadcast_kernel<true> : broadcast_kernel<false>, a,
+                         make_units(nbytes).total(), stream);
   });
 }
 
@@ -388,12 +229,10 @@ extern "C" int b200_broadcast_multi(b200_comm_t c, void *const *bufs, const size
                          [&](size_t done, size_t units) -> int {
                            a.u0 = done;
                            a.units = units;
-                           int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
-                           if (broadcast_nvls(c, units * 16))
-                             broadcast_table_kernel<true><<<g, kThreads, 0, stream>>>(c->dev(), a);
-                           else broadcast_table_kernel<false><<<g, kThreads, 0, stream>>>(c->dev(), a);
-                           B200_LAUNCH_CHECK(c);
-                           return B200_OK;
+                           return launch_staged(c,
+                                                broadcast_nvls(c, units * 16) ? broadcast_table_kernel<true>
+                                                                              : broadcast_table_kernel<false>,
+                                                a, units, stream);
                          });
 }
 
@@ -408,12 +247,7 @@ extern "C" int b200_allgather_multi(b200_comm_t c, const void *const *ins, const
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   const int n = c->world;
-  if (n == 1) {
-    for (int i = 0; i < ntensors; ++i)
-      if (nbytes[i] && outs[i] != ins[i])
-        B200_CHECK_CUDA(cudaMemcpyAsync(outs[i], ins[i], nbytes[i], cudaMemcpyDeviceToDevice, stream));
-    return B200_OK;
-  }
+  if (n == 1) return copy_list_local(outs, ins, nbytes, ntensors, stream);
   // One launch per window of at most one staging slot of each table's stream of input units.
   AGTableArgs a{};
   a.staging_bytes = c->staging_bytes;
@@ -425,10 +259,7 @@ extern "C" int b200_allgather_multi(b200_comm_t c, const void *const *ins, const
       [&](size_t done, size_t units) -> int {
         a.u0 = done;
         a.units = units;
-        int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
-        allgather_table_kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
-        B200_LAUNCH_CHECK(c);
-        return B200_OK;
+        return launch_staged(c, allgather_table_kernel, a, units, stream);
       });
 }
 

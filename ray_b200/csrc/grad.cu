@@ -14,6 +14,7 @@
 
 #include "allreduce_core.cuh"
 #include "policy.h"
+#include "staged.cuh"
 
 namespace b200 {
 
@@ -236,58 +237,28 @@ struct GradRSArgs {
   size_t staging_bytes;
 };
 
+// Unit u of every stripe: stripe q starts `stride` elements after stripe q - 1.  Stripes of a shard
+// size that is not a multiple of 4 are not all 16-byte aligned, so alignment is taken per stripe.
+template <typename W>
+struct GradStripes {
+  const GradRSArgs &a;
+  size_t u;
+  __device__ __forceinline__ uint4 load(int q) const {
+    const float *s = a.grad + size_t(q) * a.stride;
+    return load_grad_unit<W>(s, u, a.count, a.scale, is_aligned16(s));
+  }
+};
+
+// `out` may be this rank's stripe (reducescatter_push_body reduces exactly the units it pushed).
 template <typename W>
 __global__ void __launch_bounds__(kThreads, 1) grad_reducescatter_kernel(DevComm c, GradRSArgs a) {
   constexpr int E = Wire<W>::kElems;
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int n = c.world, r = c.rank;
   const size_t U = (a.count + E - 1) / E;
-  const size_t sub = U << 4;  // bytes per sub-slot
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t step = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  // push: stripe (r+i)%n goes to rank (r+i)%n, sub-slot r.  Stripes of a shard size that is not a
-  // multiple of 4 are not all 16-byte aligned, so alignment is taken per stripe.
-  for (size_t u = first; u < U; u += step) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int q = r + i;
-        if (q >= n) q -= n;
-        const float *s = a.grad + size_t(q) * a.stride;
-        v[i] = load_grad_unit<W>(s, u, a.count, a.scale, is_aligned16(s));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int q = r + i;
-        if (q >= n) q -= n;
-        st_vec(c.data[q] + off + size_t(r) * sub + (u << 4), v[i]);
-      }
-    }
-  }
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  // Every thread writes exactly the units it read from its own stripe before the barrier, so `out`
-  // may be that stripe.
-  const bool out_al = is_aligned16(a.out);
-  const char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += step) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int p = 0; p < kMaxRanks; ++p)
-      if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
-    store_grad_unit<W>(a.out, u, a.count, out_al, reduce_ranks<W, B200_SUM>(v, n));
-  }
-  finish_launch(c);
+  reducescatter_push_body(
+      c, a.staging_bytes, U, [&](size_t u) { return GradStripes<W>{a, u}; },
+      [&](size_t u, const uint4(&v)[kMaxRanks], int n) {
+        store_grad_unit<W>(a.out, u, a.count, is_aligned16(a.out), reduce_ranks<W, B200_SUM>(v, n));
+      });
 }
 
 template <typename W>
@@ -312,15 +283,10 @@ __global__ void __launch_bounds__(kLocalThreads) grad_rs_local_kernel(GradRSArgs
 
 template <typename W>
 static int launch_grad_rs(b200_comm *c, const GradRSArgs &a, cudaStream_t stream) {
-  if (c->world == 1) {
-    const size_t threads = (a.count + 3) / 4;
-    grad_rs_local_kernel<W><<<unsigned((threads + kLocalThreads - 1) / kLocalThreads), kLocalThreads, 0, stream>>>(a);
-  } else {
-    constexpr int E = Wire<W>::kElems;
-    const size_t U = (a.count + E - 1) / E;
-    const int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
-    grad_reducescatter_kernel<W><<<g, kThreads, 0, stream>>>(c->dev(), a);
-  }
+  constexpr int E = Wire<W>::kElems;
+  if (c->world > 1) return launch_staged(c, grad_reducescatter_kernel<W>, a, (a.count + E - 1) / E, stream);
+  const size_t threads = (a.count + 3) / 4;
+  grad_rs_local_kernel<W><<<unsigned((threads + kLocalThreads - 1) / kLocalThreads), kLocalThreads, 0, stream>>>(a);
   B200_LAUNCH_CHECK(c);
   return B200_OK;
 }

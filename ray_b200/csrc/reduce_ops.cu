@@ -5,11 +5,14 @@
 // caller's list and writes tensor q into sub-slot r of rank q's staging slot over
 // NVLink (the local copy-in and the transfer are the same instruction stream).  After
 // one barrier every rank reduces its n sub-slots from local HBM, rank-ascending, into
-// the caller's output tensor.  The list form (b200_reducescatter_multi) runs the same protocol
-// over windows of a packed tensor table (tensor_table.cuh).
+// the caller's output tensor.  That protocol is reducescatter_push_body (staged.cuh); the
+// tensor and list (b200_reducescatter_multi, windows of a packed tensor table, tensor_table.cuh)
+// kernels here and the FSDP gradient kernel (grad.cu) say only where a unit comes from and how
+// the reduced unit is stored.  The uneven kernel (b200_reducescatterv) writes the protocol out.
 #include <vector>
 
 #include "policy.h"
+#include "staged.cuh"
 #include "tensor_table.cuh"
 
 namespace b200 {
@@ -23,52 +26,12 @@ struct RSArgs {
 
 template <typename T, int OP>
 __global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, RSArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int n = c.world, r = c.rank;
   const Units un = make_units(a.nbytes);
-  const size_t U = un.total();
-  const size_t sub = U << 4;  // bytes per sub-slot
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  // push: tensor (r+i)%n goes to rank (r+i)%n, sub-slot r
-  for (size_t u = first; u < U; u += stride) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int q = r + i;
-        if (q >= n) q -= n;
-        v[i] = load_user_unit(a.ins[q], u, un, is_aligned16(a.ins[q]));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int q = r + i;
-        if (q >= n) q -= n;
-        st_vec(c.data[q] + off + size_t(r) * sub + (u << 4), v[i]);
-      }
-    }
-  }
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  const bool out_al = is_aligned16(a.out);
-  const char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += stride) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int p = 0; p < kMaxRanks; ++p)
-      if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
-    store_user_unit(a.out, u, un, out_al, reduce_ranks<T, OP>(v, n));
-  }
-  finish_launch(c);
+  reducescatter_push_body(
+      c, a.staging_bytes, un.total(), [&](size_t u) { return PeerParts<const char *>{a.ins, u, un}; },
+      [&](size_t u, const uint4(&v)[kMaxRanks], int n) {
+        store_user_unit(a.out, u, un, is_aligned16(a.out), reduce_ranks<T, OP>(v, n));
+      });
 }
 
 // One window of b200_reducescatterv: units [w * W, (w + 1) * W) of every rank's output part,
@@ -84,9 +47,10 @@ struct RSVArgs {
   size_t staging_bytes;
 };
 
-// reducescatter_kernel's push with a size per rank: rank r pushes the window's units of ins[q] into
-// sub-slot r of rank q's slot, crosses the barrier, then reduces its own n sub-slots rank-ascending
-// over its own part's units.  The CTA barrier pairs CTA b of every rank, so the grid (pick_blocks
+// reducescatter_push_body's protocol with a size per rank, written out: through the shared body
+// this kernel keeps its own part's size live across the barrier and needs up to 7 more registers.
+// Rank r pushes the window's units of ins[q] into sub-slot r of rank q's slot, crosses the
+// barrier, then reduces its own n sub-slots rank-ascending over its own part's units.  The CTA barrier pairs CTA b of every rank, so the grid (pick_blocks
 // on the window's largest part), the unit -> CTA mapping (grid-stride over [0, units)) and the
 // number of launches depend only on the size list, staging_bytes and the grid cap -- never on this
 // rank's own size or alignment.  A rank whose part is exhausted still launches and crosses the
@@ -153,57 +117,16 @@ struct RSTableArgs {
 };
 static_assert(fits_param_space<RSTableArgs>(), "reduce-scatter table exceeds the kernel parameter space");
 
-// reducescatter_kernel's push protocol for a window of a table (b200_reducescatter_multi): unit
-// u0 + u of entry k's input for rank q goes to byte r * units * 16 + u * 16 of rank q's slot.
 template <typename T, int OP>
 __global__ void __launch_bounds__(kThreads, 1)
     reducescatter_table_kernel(DevComm c, const __grid_constant__ RSTableArgs a) {
-  const uint32_t launch = c.st->launch_ctr;
-  const uint32_t ep = launch * 4u;
-  const int n = c.world, r = c.rank;
-  const size_t U = a.units;
-  const size_t sub = U << 4;  // bytes per sub-slot
-  const size_t off = staging_slot_offset(launch, a.staging_bytes);
-  const size_t stride = size_t(gridDim.x) * kThreads;
-  const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
-
-  for (size_t u = first; u < U; u += stride) {
-    const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
-    const size_t lu = a.u0 + u - a.t.ustart[k];
-    const Units un = make_units(a.t.nbytes[k]);
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int q = r + i;
-        if (q >= n) q -= n;
-        v[i] = load_user_unit(a.ins[k][q], lu, un, is_aligned16(a.ins[k][q]));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < kMaxRanks; ++i) {
-      if (i < n) {
-        int q = r + i;
-        if (q >= n) q -= n;
-        st_vec(c.data[q] + off + size_t(r) * sub + (u << 4), v[i]);
-      }
-    }
-  }
-
-  if (!cta_barrier_all(c, ep + 1)) {
-    finish_launch(c);
-    return;
-  }
-
-  const char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += stride) {
-    uint4 v[kMaxRanks];
-#pragma unroll
-    for (int p = 0; p < kMaxRanks; ++p)
-      if (p < n) v[p] = ld_peer(mine + size_t(p) * sub + (u << 4));
-    table_store_unit(a.t, a.u0 + u, reduce_ranks<T, OP>(v, n));
-  }
-  finish_launch(c);
+  reducescatter_push_body(
+      c, a.staging_bytes, a.units,
+      [&](size_t u) {
+        const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
+        return PeerParts<const char *>{a.ins[k], a.u0 + u - a.t.ustart[k], make_units(a.t.nbytes[k])};
+      },
+      [&](size_t u, const uint4(&v)[kMaxRanks], int n) { table_store_unit(a.t, a.u0 + u, reduce_ranks<T, OP>(v, n)); });
 }
 
 struct ReduceArgs {
@@ -246,24 +169,6 @@ __global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceAr
   finish_launch(c);
 }
 
-template <typename T, int OP>
-static int launch_rs(b200_comm *c, const RSArgs &a, cudaStream_t stream) {
-  const size_t U = make_units(a.nbytes).total();
-  int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
-  reducescatter_kernel<T, OP><<<g, kThreads, 0, stream>>>(c->dev(), a);
-  B200_LAUNCH_CHECK(c);
-  return B200_OK;
-}
-
-template <typename T, int OP>
-static int launch_reduce(b200_comm *c, const ReduceArgs &a, cudaStream_t stream) {
-  const size_t U = make_units(a.nbytes).total();
-  int g = pick_blocks(c, (U + kThreads - 1) / kThreads, c->sm_count);
-  reduce_kernel<T, OP><<<g, kThreads, 0, stream>>>(c->dev(), a);
-  B200_LAUNCH_CHECK(c);
-  return B200_OK;
-}
-
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
 const void *reduce_ops_module_anchor() { return reinterpret_cast<const void *>(&reducescatter_kernel<float, B200_SUM>); }
 
@@ -298,9 +203,9 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
     a.out = static_cast<char *>(out) + done;
     a.nbytes = nbytes;
     a.staging_bytes = c->staging_bytes;
-    int rc2 = B200_OK;
-    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc2 = launch_rs<T, OP>(c, a, stream); }));
-    return rc2;
+    B200_DISPATCH_DTYPE(dtype, T,
+                        B200_DISPATCH_OP(op, OP, { return launch_staged(c, reducescatter_kernel<T, OP>, a,
+                                                                        make_units(nbytes).total(), stream); }));
   });
 }
 
@@ -336,10 +241,7 @@ extern "C" int b200_reducescatterv(b200_comm_t c, const void *const *ins, const 
     }
     a.out = a.nbytes[c->rank] ? static_cast<char *>(out) + (u0 << 4) : nullptr;
     a.units = units;
-    int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
-    kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
-    B200_LAUNCH_CHECK(c);
-    return B200_OK;
+    return launch_staged(c, kernel, a, units, stream);
   });
 }
 
@@ -359,12 +261,7 @@ extern "C" int b200_reducescatter_multi(b200_comm_t c, const void *const *ins, v
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   const int n = c->world;
-  if (n == 1) {
-    for (int i = 0; i < ntensors; ++i)
-      if (nbytes[i] && outs[i] != ins[i])
-        B200_CHECK_CUDA(cudaMemcpyAsync(outs[i], ins[i], nbytes[i], cudaMemcpyDeviceToDevice, stream));
-    return B200_OK;
-  }
+  if (n == 1) return copy_list_local(outs, ins, nbytes.data(), ntensors, stream);
   void (*kernel)(DevComm, const RSTableArgs) = nullptr;
   B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatter_table_kernel<T, OP>; }));
   // One launch per window of each table's stream of output units; the n sub-slots of a window
@@ -379,10 +276,7 @@ extern "C" int b200_reducescatter_multi(b200_comm_t c, const void *const *ins, v
       [&](size_t done, size_t units) -> int {
         a.u0 = done;
         a.units = units;
-        int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
-        kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
-        B200_LAUNCH_CHECK(c);
-        return B200_OK;
+        return launch_staged(c, kernel, a, units, stream);
       });
 }
 
@@ -399,9 +293,9 @@ extern "C" int b200_reduce(b200_comm_t c, void *buf, size_t count, int dtype, in
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   return for_each_piece(count * es, c->staging_bytes, [&](size_t done, size_t nbytes) -> int {
-    ReduceArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
-    int rc2 = B200_OK;
-    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { rc2 = launch_reduce<T, OP>(c, a, stream); }));
-    return rc2;
+    const ReduceArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
+    B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, {
+                          return launch_staged(c, reduce_kernel<T, OP>, a, make_units(nbytes).total(), stream);
+                        }));
   });
 }

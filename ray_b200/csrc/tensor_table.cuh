@@ -1,7 +1,8 @@
 // tensor_table.cuh — tensor lists as one packed stream of 16-byte units, shared by the list
 // point-to-point calls (p2p.cu: b200_send_multi / b200_recv_multi / b200_get_multi), the list
 // broadcast and all-gather (copy_ops.cu: b200_broadcast_multi, b200_allgather_multi) and the list
-// reduce-scatter (reduce_ops.cu: b200_reducescatter_multi).
+// reduce-scatter (reduce_ops.cu: b200_reducescatter_multi).  The list collectives run the staged
+// protocols of staged.cuh over a window of the stream; this file holds only the table.
 //
 // A table's tensors form ONE packed stream: tensor i occupies 16-byte units [ustart[i], ustart[i+1])
 // with ustart[i+1] = ustart[i] + ceil(nbytes[i] / 16), so no unit mixes two tensors.  The padding of
@@ -20,8 +21,10 @@ struct P2PTable {
   unsigned long long ustart[kP2PTableMax + 1];
 };
 
-// the entry that owns unit u of a table's packed message (ustart strictly increasing)
-__device__ __forceinline__ int table_entry(const unsigned long long *start, int count, size_t u) {
+// the entry that owns unit u of a table's packed message (start strictly increasing); also the
+// all-reduce's TensorTable (allreduce_core.cuh), whose starts are unsigned int
+template <typename S>
+__device__ __forceinline__ int table_entry(const S *start, int count, size_t u) {
   int lo = 0, hi = count - 1;
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -76,6 +79,15 @@ inline int check_list_rank_ptrs(const void *const *ptrs, const size_t *nbytes, i
         set_error("%s %d of tensor %d is null but has %zu bytes", what, p, i, nbytes[i]);
         return B200_ERR_INVALID;
       }
+  return B200_OK;
+}
+
+// World 1 of the list all-gather and reduce-scatter: entry i of srcs is copied to dsts[i].
+inline int copy_list_local(void *const *dsts, const void *const *srcs, const size_t *nbytes, int ntensors,
+                           cudaStream_t stream) {
+  for (int i = 0; i < ntensors; ++i)
+    if (nbytes[i] && dsts[i] != srcs[i])
+      B200_CHECK_CUDA(cudaMemcpyAsync(dsts[i], srcs[i], nbytes[i], cudaMemcpyDeviceToDevice, stream));
   return B200_OK;
 }
 
