@@ -74,6 +74,23 @@ typedef enum {
   B200_OP_COUNT = 5
 } b200_op_t;
 
+/* PREMUL_SUM (ncclRedOpCreatePreMulSum / ncclRedOpDestroy): an op handle, passed as the `op` of
+ * b200_allreduce, b200_allreduce_multi, b200_reduce, b200_reducescatter, b200_reducescatterv and
+ * b200_reducescatter_multi, that reduces as SUM over y_r = round_T(x_r * factor): each rank scales
+ * its input as it reads it, before anything reaches a peer, computing the product in double for
+ * f64 and in fp32 for f32 / f16 / bf16, rounded once to T.  The result is therefore bit-identical
+ * to SUM on y through the same entry and algorithm.  dtype: the one operand dtype the op may be
+ * used with (f16, bf16, f32, f64; integer dtypes return B200_ERR_UNSUPPORTED).  scalar points at
+ * one value of that dtype.  residence 0: *scalar is read now.  residence 1: scalar is a device
+ * pointer that every kernel using the op reads when it runs, so a captured graph replays with the
+ * value it holds then; keeping it alive until those kernels ran is the caller's job.  Handles lie
+ * outside [0, B200_OP_COUNT); a handle used with another dtype returns B200_ERR_INVALID, and a
+ * destroyed or never-created one B200_ERR_UNSUPPORTED, as any unknown op does.  Destroying an op
+ * after calls were enqueued with it is allowed: they copied the factor into their arguments.  At
+ * world size 1 the entries write y (one scale kernel per tensor) instead of copying. */
+int b200_op_create_premul(b200_comm_t comm, const void *scalar, int dtype, int residence, int *op);
+int b200_op_destroy(b200_comm_t comm, int op);
+
 /* Algorithm selector for b200_allreduce (B200_ALGO_AUTO picks by size / dtype / op). */
 typedef enum {
   B200_ALGO_AUTO = 0,
@@ -153,7 +170,12 @@ void b200_pool_free(void *ptr, size_t size, int device, void *stream);
 /* ---- collectives ------------------------------------------------------------ */
 
 /* out[i] = op over ranks of in[i]; in == out allowed (in place).
- * Replaces ncclAllReduce at nccl_collective_group.py:200-207 and nccl_group.py:293-312. */
+ * Replaces ncclAllReduce at nccl_collective_group.py:200-207 and nccl_group.py:293-312.
+ * A PREMUL_SUM op runs on LL, ONESHOT, TWOSHOT and NVLS wherever SUM does, with SUM's launches;
+ * B200_ALGO_PIPE returns B200_ERR_UNSUPPORTED before anything is launched.  AUTO makes SUM's choice,
+ * except where SUM would take the pipelined kernels or the zero-copy symmetric-heap form, neither
+ * of which reads the input into registers: there it takes the staged two-shot kernel, NVLS when
+ * SUM's NVLS rule holds for the message. */
 int b200_allreduce(b200_comm_t comm, const void *in, void *out, size_t count,
                    int dtype, int op, int algo, void *stream);
 
@@ -166,7 +188,8 @@ int b200_allgather(b200_comm_t comm, const void *in, void *const *outs, size_t c
 
 /* out = op over ranks q of (rank q's ins[this rank]).  Reads the caller's n input
  * tensors directly: replaces the n device copies + ncclReduceScatter at
- * nccl_collective_group.py:321-360 and nccl_group.py:314-333. */
+ * nccl_collective_group.py:321-360 and nccl_group.py:314-333.  Takes a PREMUL_SUM op: each input
+ * unit is scaled as it is pushed. */
 int b200_reducescatter(b200_comm_t comm, const void *const *ins, void *out, size_t count,
                        int dtype, int op, void *stream);
 
@@ -203,8 +226,8 @@ int b200_allgatherv(b200_comm_t comm, const void *in, const size_t *counts, void
  * stream order.  A count list that differs between ranks breaks the contract, as mismatched send /
  * recv sizes do; it cannot be detected locally.  Refused calls (NULL arrays, a NULL pointer with a
  * non-zero count) launch nothing and return B200_ERR_INVALID; a bad dtype or op returns
- * B200_ERR_UNSUPPORTED.  Replaces ProcessGroupNCCL's reduce-scatter of unequal sizes, a coalesced
- * group of one ncclReduce per rank. */
+ * B200_ERR_UNSUPPORTED.  Takes a PREMUL_SUM op, with the same launches.  Replaces ProcessGroupNCCL's
+ * reduce-scatter of unequal sizes, a coalesced group of one ncclReduce per rank. */
 int b200_reducescatterv(b200_comm_t comm, const void *const *ins, const size_t *counts, void *out,
                         int dtype, int op, void *stream);
 
@@ -213,7 +236,8 @@ int b200_reducescatterv(b200_comm_t comm, const void *const *ins, const size_t *
 int b200_broadcast(b200_comm_t comm, void *buf, size_t count, int dtype, int root,
                    void *stream);
 
-/* Only root's buffer is modified.  Replaces ncclReduce at nccl_collective_group.py:231-255. */
+/* Only root's buffer is modified.  Replaces ncclReduce at nccl_collective_group.py:231-255.
+ * Takes a PREMUL_SUM op (every rank's buffer is scaled as it is staged, none is written but root's). */
 int b200_reduce(b200_comm_t comm, void *buf, size_t count, int dtype, int op, int root,
                 void *stream);
 
@@ -342,8 +366,9 @@ int b200_allgather_multi(b200_comm_t comm, const void *const *ins, const size_t 
  * every other collective.  Refused calls (ntensors < 0, NULL arrays with ntensors > 0, a NULL pointer
  * with a non-zero count) launch nothing and return B200_ERR_INVALID; a bad dtype or op returns
  * B200_ERR_UNSUPPORTED as in b200_reducescatter.  At world size 1 every entry that is not in place is
- * copied with cudaMemcpyAsync (AVG over one rank is the identity).  Replaces one ncclReduceScatter
- * per tensor of c10d's coalesced reduce-scatter (reduce_scatter_tensor_coalesced). */
+ * copied with cudaMemcpyAsync (AVG over one rank is the identity).  Takes a PREMUL_SUM op, with the
+ * same launches.  Replaces one ncclReduceScatter per tensor of c10d's coalesced reduce-scatter
+ * (reduce_scatter_tensor_coalesced). */
 int b200_reducescatter_multi(b200_comm_t comm, const void *const *ins, void *const *outs,
                              const size_t *counts, int ntensors, int dtype, int op, void *stream);
 
@@ -368,7 +393,8 @@ int b200_grad_reducescatter(b200_comm_t comm, const float *grad, float *out, siz
 
 /* Multi-tensor all-reduce (SURVEY K9): reduces `ntensors` same-dtype tensors as one
  * message without a host-side flatten (replaces parameters_to_vector + views at
- * dag/collective_node.py:220-232).  ptrs/counts are host arrays. */
+ * dag/collective_node.py:220-232).  ptrs/counts are host arrays.  Takes a PREMUL_SUM op: the
+ * table kernel scales as it gathers, and tensors it does not take go through b200_allreduce. */
 int b200_allreduce_multi(b200_comm_t comm, void *const *ptrs, const size_t *counts,
                          int ntensors, int dtype, int op, void *stream);
 

@@ -30,6 +30,8 @@ ERR_TOO_LARGE = -7
 U8, I8, I32, U32, I64, U64, F16, BF16, F32, F64 = range(10)
 # reduce ops (b200_op_t) -- same numbering as ray.util.collective.types.ReduceOp
 SUM, PROD, MIN, MAX, AVG = range(5)
+# b200_op_create_premul residence
+PREMUL_HOST, PREMUL_DEVICE = 0, 1
 # tuning parameters (b200_param_t)
 (PARAM_ONESHOT_MAX_BYTES, PARAM_NVLS_MIN_WORLD, PARAM_NVLS_CTAS, PARAM_LL_MAX_BYTES, PARAM_PIPE_MIN_BYTES,
  PARAM_PIPE_CHUNK_BYTES, PARAM_PIPE_COPY_CTAS, PARAM_PIPE_RED_CTAS, PARAM_P2P_BULK_MIN_CHUNK,
@@ -82,6 +84,8 @@ SIGNATURES = {
     "b200_pool_bind": (c_int, [c_void_p]),
     "b200_pool_alloc": (c_void_p, [c_size_t, c_int, c_void_p]),
     "b200_pool_free": (None, [c_void_p, c_size_t, c_int, c_void_p]),
+    "b200_op_create_premul": (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(c_int)]),
+    "b200_op_destroy": (c_int, [c_void_p, c_int]),
     "b200_allreduce": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
     "b200_allgather": (c_int, [c_void_p, c_void_p, POINTER(c_void_p), c_size_t, c_int, c_void_p]),
     "b200_reducescatter": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_size_t, c_int, c_int, c_void_p]),

@@ -61,6 +61,39 @@ def _tensor_list(tensors: Sequence[torch.Tensor]):
     return ptrs, sizes
 
 
+PREMUL_DTYPES = (torch.float16, torch.bfloat16, torch.float32, torch.float64)
+
+
+class PremulSum:
+    """c10d's ``PREMUL_SUM(factor)``, usable as the ``op`` of every reducing ``B200Comm`` method:
+    SUM over ``round_T(x_r * factor)``, each rank's input scaled as the kernel reads it.
+
+    ``factor`` is a float or a one-element tensor.  A CPU tensor is read now, with ``.item()``.  A
+    CUDA tensor must have the operand's dtype and is read by the kernels when they run, so the host
+    never synchronises and a captured CUDA graph replays with the value it holds at replay time.
+    A float factor is rounded to the operand's dtype, as ProcessGroupNCCL does."""
+
+    def __init__(self, factor):
+        if isinstance(factor, torch.Tensor):
+            if factor.numel() != 1:
+                raise RuntimeError(f"PREMUL_SUM factor must have exactly one element, got {factor.numel()}")
+            if not factor.is_cuda:
+                factor = float(factor.item())
+        elif isinstance(factor, (int, float)) and not isinstance(factor, bool):
+            factor = float(factor)
+        else:
+            raise RuntimeError(f"PREMUL_SUM factor must be a float or a one-element tensor, got {type(factor)}")
+        self.factor = factor
+
+    @property
+    def device_factor(self) -> Optional[torch.Tensor]:
+        """The CUDA factor tensor the kernels read, or None for a host factor."""
+        return self.factor if isinstance(self.factor, torch.Tensor) else None
+
+    def __repr__(self) -> str:
+        return f"PremulSum({self.factor!r})"
+
+
 class SymmetricTensorHolder:
     """Exposes a slice of the symmetric heap through __cuda_array_interface__."""
 
@@ -228,6 +261,35 @@ class B200Comm:
     def symm_contains(self, t: torch.Tensor) -> bool:
         return bool(self._lib.b200_symm_contains(self._h, t.data_ptr(), t.numel() * t.element_size()))
 
+    def _with_op(self, op, dtype: torch.dtype, enqueue) -> None:
+        """``enqueue(op_code)``.  A ``PremulSum`` becomes a native op for ``dtype`` that lives for this
+        call only: the kernels copy the factor (or its device address) into their arguments."""
+        if not isinstance(op, PremulSum):
+            enqueue(int(op))
+            return
+        if dtype not in PREMUL_DTYPES:
+            # ProcessGroupNCCL's refusal for an integer (or bool) operand
+            raise RuntimeError(f"Cannot use ReduceOp.PREMUL_SUM with {dtype}: "
+                               "PreMulSum Data type must be half, float, bfloat16 or double")
+        f = op.device_factor
+        handle = ctypes.c_int()
+        if f is not None:
+            if f.dtype != dtype or f.numel() != 1:
+                raise RuntimeError(f"PREMUL_SUM factor tensor must hold one {dtype} element, got "
+                                   f"{f.numel()} of {f.dtype}")
+            N.check(self._lib.b200_op_create_premul(self._h, f.data_ptr(), dtype_code(dtype), N.PREMUL_DEVICE,
+                                                    ctypes.byref(handle)))
+        else:
+            host = torch.tensor([op.factor], dtype=dtype)
+            N.check(self._lib.b200_op_create_premul(self._h, host.data_ptr(), dtype_code(dtype), N.PREMUL_HOST,
+                                                    ctypes.byref(handle)))
+        try:
+            enqueue(handle.value)
+        finally:
+            self._lib.b200_op_destroy(self._h, handle.value)
+        if f is not None:
+            f.record_stream(torch.cuda.current_stream(self.device))
+
     # ------------------------------------------------------------------ collectives
     def allreduce(self, tensor: torch.Tensor, op: int = N.SUM, out: Optional[torch.Tensor] = None,
                   algo: int = N.ALGO_AUTO) -> None:
@@ -237,8 +299,9 @@ class B200Comm:
             _check_cuda_contiguous(out, "output tensor")
             if out.dtype != tensor.dtype or out.numel() != tensor.numel():
                 raise RuntimeError("allreduce output must match the input's dtype and size")
-        N.check(self._lib.b200_allreduce(self._h, tensor.data_ptr(), out.data_ptr(), tensor.numel(),
-                                         dtype_code(tensor.dtype), int(op), int(algo), self._stream()))
+        self._with_op(op, tensor.dtype, lambda code: N.check(self._lib.b200_allreduce(
+            self._h, tensor.data_ptr(), out.data_ptr(), tensor.numel(), dtype_code(tensor.dtype), code, int(algo),
+            self._stream())))
 
     def allgather(self, outs: Sequence[torch.Tensor], tensor: torch.Tensor) -> None:
         _check_cuda_contiguous(tensor)
@@ -276,8 +339,8 @@ class B200Comm:
             if t.dtype != out.dtype or t.numel() != out.numel():
                 raise RuntimeError("All tensor operands to reducescatter must have the same dtype and size.")
             arr[i] = t.data_ptr()
-        N.check(self._lib.b200_reducescatter(self._h, arr, out.data_ptr(), out.numel(),
-                                             dtype_code(out.dtype), int(op), self._stream()))
+        self._with_op(op, out.dtype, lambda code: N.check(self._lib.b200_reducescatter(
+            self._h, arr, out.data_ptr(), out.numel(), dtype_code(out.dtype), code, self._stream())))
 
     def reducescatter_from(self, out: torch.Tensor, tensor: torch.Tensor, op: int = N.SUM) -> None:
         """out = reduce over ranks of this rank's 1/world slice of ``tensor`` along dim 0
@@ -290,8 +353,8 @@ class B200Comm:
         step = out.numel() * out.element_size()
         for p in range(self.world_size):
             arr[p] = tensor.data_ptr() + p * step
-        N.check(self._lib.b200_reducescatter(self._h, arr, out.data_ptr(), out.numel(),
-                                             dtype_code(out.dtype), int(op), self._stream()))
+        self._with_op(op, out.dtype, lambda code: N.check(self._lib.b200_reducescatter(
+            self._h, arr, out.data_ptr(), out.numel(), dtype_code(out.dtype), code, self._stream())))
 
     def _uneven_parts(self, parts: Sequence[torch.Tensor], own: torch.Tensor, what: str, own_what: str):
         """(pointer array, count array) of the world_size parts of an uneven all-gather or
@@ -327,8 +390,8 @@ class B200Comm:
         ``reducescatter``'s launches."""
         _check_cuda_contiguous(out, "output tensor")
         ptrs, counts = self._uneven_parts(ins, out, "reducescatterv", "output has")
-        N.check(self._lib.b200_reducescatterv(self._h, ptrs, counts, out.data_ptr(), dtype_code(out.dtype),
-                                              int(op), self._stream()))
+        self._with_op(op, out.dtype, lambda code: N.check(self._lib.b200_reducescatterv(
+            self._h, ptrs, counts, out.data_ptr(), dtype_code(out.dtype), code, self._stream())))
 
     def allgather_multi(self, out_lists: Sequence[Sequence[torch.Tensor]], tensors: Sequence[torch.Tensor]) -> None:
         """``allgather`` of a list of tensors (any dtypes): ``out_lists[i][p]`` receives rank p's
@@ -381,8 +444,8 @@ class B200Comm:
             counts[i] = o.numel()
         if not outs:
             return
-        N.check(self._lib.b200_reducescatter_multi(self._h, ins, ptrs, counts, len(outs), dtype_code(outs[0].dtype),
-                                                   int(op), self._stream()))
+        self._with_op(op, outs[0].dtype, lambda code: N.check(self._lib.b200_reducescatter_multi(
+            self._h, ins, ptrs, counts, len(outs), dtype_code(outs[0].dtype), code, self._stream())))
 
     def _check_rs_outputs(self, outs: Sequence[torch.Tensor], n_in: int) -> None:
         if len(outs) != n_in:
@@ -445,8 +508,8 @@ class B200Comm:
 
     def reduce(self, tensor: torch.Tensor, root: int = 0, op: int = N.SUM) -> None:
         _check_cuda_contiguous(tensor)
-        N.check(self._lib.b200_reduce(self._h, tensor.data_ptr(), tensor.numel(),
-                                      dtype_code(tensor.dtype), int(op), int(root), self._stream()))
+        self._with_op(op, tensor.dtype, lambda code: N.check(self._lib.b200_reduce(
+            self._h, tensor.data_ptr(), tensor.numel(), dtype_code(tensor.dtype), code, int(root), self._stream())))
 
     def barrier(self) -> None:
         N.check(self._lib.b200_barrier(self._h, self._stream()))
@@ -623,8 +686,8 @@ class B200Comm:
                 raise ValueError("Expected all input tensors to have the same dtype")
             ptrs[i] = t.data_ptr()
             counts[i] = t.numel()
-        N.check(self._lib.b200_allreduce_multi(self._h, ptrs, counts, len(tensors), dtype_code(dt),
-                                               int(op), self._stream()))
+        self._with_op(op, dt, lambda code: N.check(self._lib.b200_allreduce_multi(
+            self._h, ptrs, counts, len(tensors), dtype_code(dt), code, self._stream())))
 
     # ------------------------------------------------------------------ lifecycle
     def abort(self) -> None:

@@ -37,8 +37,8 @@ struct ARArgs {
 // ---------------------------------------------------------------------------
 // one-shot
 // ---------------------------------------------------------------------------
-template <typename T, int OP>
-__global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm c, ARArgs a) {
+template <typename T, int OP, typename S>
+__device__ __forceinline__ void allreduce_oneshot_body(const DevComm &c, const ARArgs &a, const S &scale) {
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const int n = c.world, r = c.rank;
@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm 
   const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
 
   char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), load_user_unit(a.in, u, un, in_al));
+  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), scale(load_user_unit(a.in, u, un, in_al)));
 
   if (!cta_barrier_all(c, ep + 1)) {
     finish_launch(c);
@@ -65,6 +65,15 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm 
     store_user_unit(a.out, u, un, out_al, reduce_ranks<T, OP>(v, n));
   }
   finish_launch(c);
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm c, ARArgs a) {
+  allreduce_oneshot_body<T, OP>(c, a, NoScale{});
+}
+// PREMUL_SUM (OP = kOpPremulSum): the same kernel with the input scaled at stage-in
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_oneshot_kernel(DevComm c, ARArgs a, PremulArg f) {
+  allreduce_oneshot_body<T, OP>(c, a, Premul<T>(f));
 }
 
 // ---------------------------------------------------------------------------
@@ -86,8 +95,9 @@ __device__ __forceinline__ uint4 ll_load(const void *p) {
   return v;
 }
 
-template <typename T, int OP>
-__global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(DevComm c, ARArgs a) {
+// `a` and `scale` by value: taken by reference, the plain 4-byte kernels schedule four moves differently
+template <typename T, int OP, typename S>
+__device__ __forceinline__ void allreduce_ll_body(const DevComm &c, ARArgs a, S scale) {
   using Tr = Traits<T>;
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t flag = launch + 1u;  // never 0, never equal to what the slot held two launches ago
@@ -97,7 +107,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(DevComm c, AR
   const size_t u = size_t(blockIdx.x) * kThreads + threadIdx.x;
   const size_t par_off = (launch & 1u) ? size_t(kMaxRanks) * kLLSlotBytes : 0;
   if (u < U) {
-    const uint4 mine = load_user_unit(a.in, u, un, is_aligned16(a.in));
+    const uint4 mine = scale(load_user_unit(a.in, u, un, is_aligned16(a.in)));
     // push (start with the next rank so the eight peers are not hit in lock step)
 #pragma unroll
     for (int i = 1; i < kMaxRanks; ++i) {
@@ -152,12 +162,21 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(DevComm c, AR
   }
   finish_launch(c);
 }
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(DevComm c, ARArgs a) {
+  allreduce_ll_body<T, OP>(c, a, NoScale{});
+}
+// PREMUL_SUM: the scaled unit is what is pushed to the peers and reduced locally
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_ll_kernel(DevComm c, ARArgs a, PremulArg f) {
+  allreduce_ll_body<T, OP>(c, a, Premul<T>(f));
+}
 
 // ---------------------------------------------------------------------------
 // two-shot / NVLS
 // ---------------------------------------------------------------------------
-template <typename T, int OP, bool NVLS>
-__global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(DevComm c, ARArgs a) {
+template <typename T, int OP, bool NVLS, typename S>
+__device__ __forceinline__ void allreduce_twoshot_body(const DevComm &c, const ARArgs &a, const S &scale) {
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const Units un = make_units(a.nbytes);
@@ -168,7 +187,7 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(DevComm 
   // phase 0: stage this CTA's rows into the local symmetric slot
   if (staged) {
     const bool in_al = is_aligned16(a.in);
-    stage_in_rows(c, off, g, [&](size_t u) { return load_user_unit(a.in, u, un, in_al); });
+    stage_in_rows(c, off, g, [&](size_t u) { return scale(load_user_unit(a.in, u, un, in_al)); });
   }
   // phase 1: reduce the units this rank owns, publish to every peer
   if (!reduce_phase<T, OP, NVLS>(c, ep, off, g, a.red_ctas)) {
@@ -182,15 +201,24 @@ __global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(DevComm 
   }
   finish_launch(c);
 }
+template <typename T, int OP, bool NVLS>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(DevComm c, ARArgs a) {
+  allreduce_twoshot_body<T, OP, NVLS>(c, a, NoScale{});
+}
+// PREMUL_SUM: always staged (the zero-copy form has no stage-in to scale at); NVLS reduces as SUM
+template <typename T, int OP, bool NVLS>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_twoshot_kernel(DevComm c, ARArgs a, PremulArg f) {
+  allreduce_twoshot_body<T, OP, NVLS>(c, a, Premul<T>(f));
+}
 
 // ---------------------------------------------------------------------------
 // multi-tensor (SURVEY K9): the same three phases, but stage-in gathers from / stage-out
 // scatters to a table of tensors, so a list of tensors is reduced as ONE message in ONE
 // launch with no host-side flatten (dag/collective_node.py:220-232 uses parameters_to_vector).
 // ---------------------------------------------------------------------------
-template <typename T, int OP, bool NVLS>
-__global__ void __launch_bounds__(kThreads, 1)
-allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t staging_bytes, int red_ctas) {
+template <typename T, int OP, bool NVLS, typename S>
+__device__ __forceinline__ void allreduce_multi_body(const DevComm &c, const TensorTable &tb, size_t staging_bytes,
+                                                     int red_ctas, const S &scale) {
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const RowGeom g = make_rows(tb.ustart[tb.count], c.world);
@@ -198,7 +226,7 @@ allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t
 
   stage_in_rows(c, off, g, [&](size_t u) {
     const int i = table_entry(tb.ustart, tb.count, u);
-    return load_user_unit(tb.ptr[i], u - tb.ustart[i], make_units(tb.nbytes[i]), is_aligned16(tb.ptr[i]));
+    return scale(load_user_unit(tb.ptr[i], u - tb.ustart[i], make_units(tb.nbytes[i]), is_aligned16(tb.ptr[i])));
   });
   if (!reduce_phase<T, OP, NVLS>(c, ep, off, g, red_ctas)) {
     finish_launch(c);
@@ -210,23 +238,35 @@ allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t
   });
   finish_launch(c);
 }
+template <typename T, int OP, bool NVLS>
+__global__ void __launch_bounds__(kThreads, 1)
+allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb, size_t staging_bytes, int red_ctas) {
+  allreduce_multi_body<T, OP, NVLS>(c, tb, staging_bytes, red_ctas, NoScale{});
+}
+// PREMUL_SUM: the table gather scales each unit
+template <typename T, int OP, bool NVLS>
+__global__ void __launch_bounds__(kThreads, 1) allreduce_multi_kernel(DevComm c, const __grid_constant__ TensorTable tb,
+                                                                      size_t staging_bytes, int red_ctas, PremulArg f) {
+  allreduce_multi_body<T, OP, NVLS>(c, tb, staging_bytes, red_ctas, Premul<T>(f));
+}
 
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-template <typename T, int OP>
+// `f...` is empty for the plain ops and the PremulArg for OP = kOpPremulSum, which picks that kernel.
+template <typename T, int OP, typename... F>
 static int launch_allreduce(b200_comm *c, const char *in, char *out, size_t nbytes, int algo,
-                            long long sym_off, cudaStream_t stream) {
+                            long long sym_off, cudaStream_t stream, const F &...f) {
   DevComm dc = c->dev();
   ARArgs a{in, out, nbytes, c->staging_bytes, sym_off, 0};
   const size_t U = make_units(nbytes).total();
   if (algo == B200_ALGO_LL) {
     a.sym_off = -1;
-    allreduce_ll_kernel<T, OP><<<int((U + kThreads - 1) / kThreads), kThreads, 0, stream>>>(dc, a);
+    allreduce_ll_kernel<T, OP><<<int((U + kThreads - 1) / kThreads), kThreads, 0, stream>>>(dc, a, f...);
   } else if (algo == B200_ALGO_ONESHOT) {
     a.sym_off = -1;
     int g = pick_blocks(c, (U + kThreads - 1) / kThreads, 32);
-    allreduce_oneshot_kernel<T, OP><<<g, kThreads, 0, stream>>>(dc, a);
+    allreduce_oneshot_kernel<T, OP><<<g, kThreads, 0, stream>>>(dc, a, f...);
   } else {
     const size_t rows = (U + size_t(c->world) * kThreads - 1) / (size_t(c->world) * kThreads);
     int g = pick_blocks(c, rows, c->sm_count);
@@ -237,22 +277,48 @@ static int launch_allreduce(b200_comm *c, const char *in, char *out, size_t nbyt
         if (g > cap && c->forced_blocks == 0) g = cap;
         a.red_ctas = 0;
       }
-      if constexpr (Multimem<T>::kSum && (OP == B200_SUM || OP == B200_AVG)) {
-        allreduce_twoshot_kernel<T, OP, true><<<g, kThreads, 0, stream>>>(dc, a);
+      if constexpr (Multimem<T>::kSum && (OP == B200_SUM || OP == B200_AVG || OP == kOpPremulSum)) {
+        allreduce_twoshot_kernel<T, OP, true><<<g, kThreads, 0, stream>>>(dc, a, f...);
       } else {
         set_error("NVLS all-reduce supports SUM/AVG on f32/f16/bf16 only");
         return B200_ERR_UNSUPPORTED;
       }
     } else {
-      allreduce_twoshot_kernel<T, OP, false><<<g, kThreads, 0, stream>>>(dc, a);
+      allreduce_twoshot_kernel<T, OP, false><<<g, kThreads, 0, stream>>>(dc, a, f...);
     }
   }
   B200_LAUNCH_CHECK(c);
   return B200_OK;
 }
 
+// World size 1 of the PREMUL_SUM entries: out = round_T(in * factor), unit by unit, so in place works
+// and either pointer may have any alignment.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) premul_scale_kernel(const char *in, char *out, size_t nbytes,
+                                                                PremulArg f) {
+  const Premul<T> scale(f);
+  const Units un = make_units(nbytes);
+  const bool in_al = is_aligned16(in), out_al = is_aligned16(out);
+  const size_t stride = size_t(gridDim.x) * kThreads;
+  for (size_t u = size_t(blockIdx.x) * kThreads + threadIdx.x; u < un.total(); u += stride)
+    store_user_unit(out, u, un, out_al, scale(load_user_unit(in, u, un, in_al)));
+}
+
+int launch_premul_scale(b200_comm *c, const void *in, void *out, size_t nbytes, int dtype, const PremulArg &f,
+                        cudaStream_t stream) {
+  if (nbytes == 0) return B200_OK;
+  B200_CHECK_CUDA(cudaSetDevice(c->device));
+  const int g = pick_blocks(c, (make_units(nbytes).total() + kThreads - 1) / kThreads, 4 * c->sm_count);
+  B200_DISPATCH_PREMUL(dtype, T, {
+    premul_scale_kernel<T><<<g, kThreads, 0, stream>>>(static_cast<const char *>(in), static_cast<char *>(out),
+                                                       nbytes, f);
+  });
+  B200_LAUNCH_CHECK(c);
+  return B200_OK;
+}
+
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
-const void *allreduce_module_anchor() { return reinterpret_cast<const void *>(&allreduce_ll_kernel<float, B200_SUM>); }
+const void *allreduce_module_anchor() { return reinterpret_cast<const void *>(static_cast<void (*)(DevComm, ARArgs)>(&allreduce_ll_kernel<float, B200_SUM>)); }
 
 }  // namespace b200
 
@@ -262,13 +328,21 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
                               int op, int algo, void *stream_) {
   int rc;
   size_t es;
-  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op))) return rc;
+  OpArg oa;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(c, op, dtype, &oa))) return rc;
+  const bool premul = oa.op == kOpPremulSum;
+  if (premul && algo == B200_ALGO_PIPE) {
+    set_error("PREMUL_SUM does not run on the pipelined all-reduce, whose copies bypass the registers it scales in");
+    return B200_ERR_UNSUPPORTED;
+  }
+  const int red_op = premul ? int(B200_SUM) : op;  // what the algorithm choice sees
   if (count == 0) return B200_OK;
   if (!in || !out) return null_tensor_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   const size_t total = count * es;
   if (c->world == 1) {
+    if (premul) return launch_premul_scale(c, in, out, total, dtype, oa.premul, stream);
     if (in != out) B200_CHECK_CUDA(cudaMemcpyAsync(out, in, total, cudaMemcpyDeviceToDevice, stream));
     return B200_OK;
   }
@@ -297,13 +371,25 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
   if (sym_off < 0 && is_aligned16(in) && is_aligned16(out) && (total & 15) == 0 && pipe_fits(c) &&
       (algo == B200_ALGO_PIPE || (algo == B200_ALGO_AUTO && total >= pipe_min_bytes(c)))) {
     if (c->world == 2) pipe_variant = PIPE_PULL;
-    else if (c->mc_active && nvls_capable(dtype, op)) pipe_variant = PIPE_NVLS;
+    else if (c->mc_active && nvls_capable(dtype, red_op)) pipe_variant = PIPE_NVLS;
     else if (algo == B200_ALGO_PIPE) pipe_variant = PIPE_PEER;  // AUTO without NVLS keeps the two-shot kernel
     if (algo == B200_ALGO_AUTO && pipe_variant >= 0 && !pipe_runs(c, PipeVariant(pipe_variant))) pipe_variant = -1;
   } else if (algo == B200_ALGO_PIPE) {
     set_error("the pipelined all-reduce needs 16-byte aligned operands outside the symmetric heap "
               "and a size that is a multiple of 16 bytes");
     return B200_ERR_UNSUPPORTED;
+  }
+
+  // PREMUL_SUM scales each rank's input as stage-in reads it.  The pipelined kernels copy it with
+  // the bulk-copy unit and the zero-copy form has no stage-in, so where SUM would take either,
+  // PREMUL_SUM takes the staged two-shot kernel: on the switch when SUM's NVLS rule holds for the
+  // message, over the peers otherwise.  Every other choice is SUM's.
+  if (premul) {
+    if (algo == B200_ALGO_AUTO && (pipe_variant >= 0 || (sym_off >= 0 && total > ll_limit(c))))
+      algo = c->mc_active && nvls_capable(dtype, red_op) && nvls_pays_off(c, total) ? B200_ALGO_NVLS
+                                                                                     : B200_ALGO_TWOSHOT;
+    pipe_variant = -1;
+    sym_off = -1;
   }
 
   // Messages larger than one staging slot are processed slot by slot.
@@ -317,13 +403,19 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
     if (a == B200_ALGO_AUTO || a == B200_ALGO_PIPE) {
       if (nbytes <= ll_limit(c)) a = B200_ALGO_LL;
       else if (sym_off < 0 && nbytes <= oneshot_limit(c)) a = B200_ALGO_ONESHOT;
-      else if (c->mc_active && nvls_capable(dtype, op) && nvls_pays_off(c, nbytes)) a = B200_ALGO_NVLS;
+      else if (c->mc_active && nvls_capable(dtype, red_op) && nvls_pays_off(c, nbytes)) a = B200_ALGO_NVLS;
       else a = B200_ALGO_TWOSHOT;
     }
     if (a == B200_ALGO_LL && nbytes > kLLMaxPayload) a = B200_ALGO_ONESHOT;
     if (a == B200_ALGO_ONESHOT && nbytes > c->staging_bytes) a = B200_ALGO_TWOSHOT;
     const long long so = sym_off >= 0 ? sym_off + (long long)done : -1;
     int rc2 = B200_OK;
+    if (premul) {
+      B200_DISPATCH_PREMUL(dtype, T, {
+        rc2 = launch_allreduce<T, kOpPremulSum>(c, src + done, dst + done, nbytes, a, so, stream, oa.premul);
+      });
+      return rc2;
+    }
     B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, {
                           rc2 = launch_allreduce<T, OP>(c, src + done, dst + done, nbytes, a, so, stream);
                         }));
@@ -333,19 +425,20 @@ extern "C" int b200_allreduce(b200_comm_t c, const void *in, void *out, size_t c
 
 // ---- multi-tensor entry ------------------------------------------------------------
 namespace b200 {
-template <typename T, int OP>
-static int launch_multi(b200_comm *c, const TensorTable &tb, cudaStream_t stream) {
+template <typename T, int OP, typename... F>
+static int launch_multi(b200_comm *c, const TensorTable &tb, cudaStream_t stream, const F &...f) {
   const size_t U = tb.ustart[tb.count];
   const size_t rows = (U + size_t(c->world) * kThreads - 1) / (size_t(c->world) * kThreads);
   int g = pick_blocks(c, rows, c->sm_count);
-  if constexpr (Multimem<T>::kSum && (OP == B200_SUM || OP == B200_AVG)) {
+  if constexpr (Multimem<T>::kSum && (OP == B200_SUM || OP == B200_AVG || OP == kOpPremulSum)) {
     if (c->mc_active) {
-      allreduce_multi_kernel<T, OP, true><<<g, kThreads, 0, stream>>>(c->dev(), tb, c->staging_bytes, nvls_ctas(c));
+      allreduce_multi_kernel<T, OP, true><<<g, kThreads, 0, stream>>>(c->dev(), tb, c->staging_bytes, nvls_ctas(c),
+                                                                      f...);
       B200_LAUNCH_CHECK(c);
       return B200_OK;
     }
   }
-  allreduce_multi_kernel<T, OP, false><<<g, kThreads, 0, stream>>>(c->dev(), tb, c->staging_bytes, 0);
+  allreduce_multi_kernel<T, OP, false><<<g, kThreads, 0, stream>>>(c->dev(), tb, c->staging_bytes, 0, f...);
   B200_LAUNCH_CHECK(c);
   return B200_OK;
 }
@@ -359,7 +452,8 @@ extern "C" int b200_allreduce_multi(b200_comm_t c, void *const *ptrs, const size
                                     int ntensors, int dtype, int op, void *stream_) {
   int rc;
   size_t es;
-  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op))) return rc;
+  OpArg oa;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(c, op, dtype, &oa))) return rc;
   if (ntensors < 0 || (ntensors > 0 && (!ptrs || !counts))) {
     set_error("invalid tensor list");
     return B200_ERR_INVALID;
@@ -405,6 +499,11 @@ extern "C" int b200_allreduce_multi(b200_comm_t c, void *const *ptrs, const size
     }
     tb.ustart[tb.count] = static_cast<unsigned int>(units);
     if (tb.count == 0) continue;
+    if (oa.op == kOpPremulSum) {
+      B200_DISPATCH_PREMUL(dtype, T, { rc = launch_multi<T, kOpPremulSum>(c, tb, stream, oa.premul); });
+      if (rc) return rc;
+      continue;
+    }
     switch (dtype) {
       case B200_F32: B200_DISPATCH_OP(op, OP, { rc = launch_multi<float, OP>(c, tb, stream); }); break;
       case B200_F64: B200_DISPATCH_OP(op, OP, { rc = launch_multi<double, OP>(c, tb, stream); }); break;
@@ -413,5 +512,47 @@ extern "C" int b200_allreduce_multi(b200_comm_t c, void *const *ptrs, const size
     }
     if (rc) return rc;
   }
+  return B200_OK;
+}
+
+// ---- PREMUL_SUM ops (ncclRedOpCreatePreMulSum / ncclRedOpDestroy) ------------------------------
+extern "C" int b200_op_create_premul(b200_comm_t c, const void *scalar, int dtype, int residence, int *op) {
+  int rc;
+  if ((rc = check_usable(c))) return rc;
+  if (!scalar || !op || (residence != 0 && residence != 1)) {
+    set_error("b200_op_create_premul: null scalar or op, or residence %d is neither 0 (host) nor 1 (device)",
+              residence);
+    return B200_ERR_INVALID;
+  }
+  double host = 0.0;
+  switch (dtype) {
+    case B200_F16: host = residence ? 0.0 : double(__half2float(*static_cast<const __half *>(scalar))); break;
+    case B200_BF16: host = residence ? 0.0 : double(__bfloat162float(*static_cast<const __nv_bfloat16 *>(scalar))); break;
+    case B200_F32: host = residence ? 0.0 : double(*static_cast<const float *>(scalar)); break;
+    case B200_F64: host = residence ? 0.0 : *static_cast<const double *>(scalar); break;
+    default: set_error("PREMUL_SUM supports f16, bf16, f32 and f64 only, not dtype %d", dtype); return B200_ERR_UNSUPPORTED;
+  }
+  for (int i = 0; i < int(sizeof(c->premul_ops) / sizeof(c->premul_ops[0])); ++i) {
+    if (c->premul_ops[i].dtype >= 0) continue;
+    c->premul_ops[i].dtype = dtype;
+    c->premul_ops[i].arg = PremulArg{host, residence ? scalar : nullptr};
+    *op = kPremulOpBase + i;
+    return B200_OK;
+  }
+  set_error("b200_op_create_premul: all %d op slots are in use", int(sizeof(c->premul_ops) / sizeof(c->premul_ops[0])));
+  return B200_ERR_INVALID;
+}
+
+extern "C" int b200_op_destroy(b200_comm_t c, int op) {
+  if (!c) {
+    set_error("null communicator");
+    return B200_ERR_INVALID;
+  }
+  const int slot = op - kPremulOpBase;
+  if (slot < 0 || slot >= int(sizeof(c->premul_ops) / sizeof(c->premul_ops[0])) || c->premul_ops[slot].dtype < 0) {
+    set_error("b200_op_destroy: %d is not a live PREMUL_SUM op", op);
+    return B200_ERR_INVALID;
+  }
+  c->premul_ops[slot].dtype = -1;
   return B200_OK;
 }

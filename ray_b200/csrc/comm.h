@@ -78,6 +78,12 @@ struct b200_comm {
   uint32_t host_barrier_seq = 0;
 
   std::atomic<uint64_t> launches{0};
+  // PREMUL_SUM ops of b200_op_create_premul: slot i is handle kPremulOpBase + i; dtype < 0 = free
+  struct PremulOp {
+    int dtype = -1;
+    b200::PremulArg arg{};
+  };
+  PremulOp premul_ops[64];
   int forced_blocks = 0;
   long long params[B200_PARAM_COUNT];  // -1 = default (the constructor sets every entry)
   int sm_count = 132;  // H100 SXM; replaced by cudaDeviceProp::multiProcessorCount at creation

@@ -268,9 +268,14 @@ __device__ __forceinline__ void finish_launch(const DevComm &c) {
 // Element traits: how a 16-byte vector of T is unpacked into an accumulator,
 // combined, and packed again.  16/8-bit floats accumulate in fp32 and round once.
 // ---------------------------------------------------------------------------
+// Internal op of the PREMUL_SUM instantiations: every rank's input is scaled as it is read
+// (Premul below), and from then on the op is SUM.  Not a b200_op_t value: callers name a PREMUL_SUM
+// op by the handle b200_op_create_premul returns.
+constexpr int kOpPremulSum = B200_OP_COUNT;
+
 template <int OP, typename A>
 __device__ __forceinline__ A combine(A a, A b) {
-  if (OP == B200_SUM || OP == B200_AVG) return a + b;
+  if (OP == B200_SUM || OP == B200_AVG || OP == kOpPremulSum) return a + b;
   if (OP == B200_PROD) return a * b;
   // MIN / MAX propagate a NaN from any rank, as np.minimum / np.maximum do: a NaN accumulator
   // survives because every comparison with it is false, and `b != b` picks up a NaN operand (it
@@ -375,6 +380,48 @@ __device__ __forceinline__ uint4 reduce_ranks(const uint4 (&v)[kMaxRanks], int n
   if (OP == B200_AVG) Tr::average(acc, n);
   return Tr::pack(acc);
 }
+
+// ---------------------------------------------------------------------------
+// PREMUL_SUM's factor.  It reaches a kernel as an argument, never as communicator state, so calls
+// with different factors may be in flight at once and a captured graph reads a device factor at
+// replay time.  The factor is a value of the operand's dtype: `host` holds it exactly, or `dev`
+// points at it and every kernel that uses the op loads it when it starts.
+// ---------------------------------------------------------------------------
+struct PremulArg {
+  double host;
+  const void *dev;  // nullptr: use `host`
+};
+
+// The scale policy of the reducing kernels: applied to each 16-byte unit of the caller's input as it
+// is read into registers, before it reaches a staging slot or a peer.  NoScale is the plain ops'.
+struct NoScale {
+  __device__ __forceinline__ uint4 operator()(uint4 v) const { return v; }
+};
+
+__device__ __forceinline__ float premul_scalar(__half h) { return __half2float(h); }
+__device__ __forceinline__ float premul_scalar(__nv_bfloat16 h) { return __bfloat162float(h); }
+__device__ __forceinline__ float premul_scalar(float f) { return f; }
+__device__ __forceinline__ double premul_scalar(double f) { return f; }
+__device__ __forceinline__ float premul_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double premul_mul(double a, double b) { return __dmul_rn(a, b); }
+
+// y = round_T(x * f): the product in double for f64, in fp32 for f32 / f16 / bf16, rounded once to
+// T.  The _rn multiplies are never contracted into an FMA with the SUM that follows, so the rank's
+// contribution is exactly y.
+template <typename T>
+struct Premul {
+  using S = decltype(premul_scalar(T()));
+  S f;
+  __device__ __forceinline__ explicit Premul(const PremulArg &a)
+      : f(a.dev ? premul_scalar(*static_cast<const T *>(a.dev)) : S(a.host)) {}
+  __device__ __forceinline__ uint4 operator()(uint4 v) const {
+    using Tr = Traits<T>;
+    typename Tr::Acc acc = Tr::unpack(v);
+#pragma unroll
+    for (int i = 0; i < Tr::kLanes; ++i) acc.v[i] = premul_mul(acc.v[i], f);
+    return Tr::pack(acc);
+  }
+};
 
 // ---------------------------------------------------------------------------
 // NVLS reduction: one instruction pulls the same 16 bytes from every rank's

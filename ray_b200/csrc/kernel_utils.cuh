@@ -78,6 +78,36 @@ inline int check_op(int op) {
   return B200_OK;
 }
 
+// Handles of b200_op_create_premul lie outside [0, B200_OP_COUNT).
+constexpr int kPremulOpBase = 0x100;
+
+// The op argument of a reducing entry: a b200_op_t value, or a live PREMUL_SUM handle, which must be
+// used with the dtype it was created for.  A handle resolves to kOpPremulSum and its factor.
+struct OpArg {
+  int op;
+  PremulArg premul;
+};
+inline int check_op(const b200_comm *c, int op, int dtype, OpArg *out) {
+  out->op = op;
+  out->premul = PremulArg{0.0, nullptr};
+  if (op >= 0 && op < B200_OP_COUNT) return B200_OK;
+  const int slot = op - kPremulOpBase;
+  const int nslots = int(sizeof(c->premul_ops) / sizeof(c->premul_ops[0]));
+  if (slot < 0 || slot >= nslots || c->premul_ops[slot].dtype < 0) return check_op(op);
+  if (c->premul_ops[slot].dtype != dtype) {
+    set_error("PREMUL_SUM op %d was created for dtype %d, used with dtype %d", op, c->premul_ops[slot].dtype, dtype);
+    return B200_ERR_INVALID;
+  }
+  out->op = kOpPremulSum;
+  out->premul = c->premul_ops[slot].arg;
+  return B200_OK;
+}
+
+// World size 1 of a PREMUL_SUM entry: out = round_T(in * factor), in place or not, any alignment
+// (allreduce.cu).  One launch.
+int launch_premul_scale(b200_comm *c, const void *in, void *out, size_t nbytes, int dtype, const PremulArg &f,
+                        cudaStream_t stream);
+
 // `what`: "root", "peer" or "source"
 inline int check_rank(const b200_comm *c, int r, const char *what) {
   if (r < 0 || r >= c->world) {
@@ -142,6 +172,18 @@ int set_dyn_smem(int device, const void *fn);
     case B200_MAX: { constexpr int OP = B200_MAX; __VA_ARGS__; break; }      \
     case B200_AVG: { constexpr int OP = B200_AVG; __VA_ARGS__; break; }      \
     default: b200::set_error("unsupported reduce op %d", int(op)); return B200_ERR_UNSUPPORTED; \
+  }
+
+// The dtypes a PREMUL_SUM op exists for (b200_op_create_premul refuses the others).  Its kernels are
+// separate instantiations with OP = kOpPremulSum and a PremulArg argument, so B200_DISPATCH_OP keeps
+// instantiating exactly the plain ops' kernels.
+#define B200_DISPATCH_PREMUL(dtype, T, ...)                                  \
+  switch (dtype) {                                                           \
+    case B200_F16: { using T = __half; __VA_ARGS__; break; }                 \
+    case B200_BF16: { using T = __nv_bfloat16; __VA_ARGS__; break; }         \
+    case B200_F32: { using T = float; __VA_ARGS__; break; }                  \
+    case B200_F64: { using T = double; __VA_ARGS__; break; }                 \
+    default: b200::set_error("PREMUL_SUM supports f16, bf16, f32 and f64 only"); return B200_ERR_UNSUPPORTED; \
   }
 
 }  // namespace b200

@@ -24,14 +24,23 @@ struct RSArgs {
   size_t staging_bytes;
 };
 
-template <typename T, int OP>
-__global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, RSArgs a) {
+// PREMUL_SUM (OP = kOpPremulSum, S = Premul<T>) scales the unit source; the body is the plain ops'.
+template <typename T, int OP, typename S>
+__device__ __forceinline__ void reducescatter_tensor_body(const DevComm &c, const RSArgs &a, const S &scale) {
   const Units un = make_units(a.nbytes);
   reducescatter_push_body(
-      c, a.staging_bytes, un.total(), [&](size_t u) { return PeerParts<const char *>{a.ins, u, un}; },
+      c, a.staging_bytes, un.total(), [&](size_t u) { return scaled(PeerParts<const char *>{a.ins, u, un}, scale); },
       [&](size_t u, const uint4(&v)[kMaxRanks], int n) {
         store_user_unit(a.out, u, un, is_aligned16(a.out), reduce_ranks<T, OP>(v, n));
       });
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, RSArgs a) {
+  reducescatter_tensor_body<T, OP>(c, a, NoScale{});
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reducescatter_kernel(DevComm c, RSArgs a, PremulArg f) {
+  reducescatter_tensor_body<T, OP>(c, a, Premul<T>(f));
 }
 
 // One window of b200_reducescatterv: units [w * W, (w + 1) * W) of every rank's output part,
@@ -55,8 +64,8 @@ struct RSVArgs {
 // number of launches depend only on the size list, staging_bytes and the grid cap -- never on this
 // rank's own size or alignment.  A rank whose part is exhausted still launches and crosses the
 // barrier (DESIGN.md §3).  Every output element has n contributions, so AVG divides by n.
-template <typename T, int OP>
-__global__ void __launch_bounds__(kThreads, 1) reducescatterv_kernel(DevComm c, RSVArgs a) {
+template <typename T, int OP, typename S>
+__device__ __forceinline__ void reducescatterv_body(const DevComm &c, const RSVArgs &a, const S &scale) {
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const int n = c.world, r = c.rank;
@@ -74,7 +83,7 @@ __global__ void __launch_bounds__(kThreads, 1) reducescatterv_kernel(DevComm c, 
         int q = r + i;
         if (q >= n) q -= n;
         const Units un = make_units(a.nbytes[q]);
-        if (u < un.total()) v[i] = load_user_unit(a.ins[q], u, un, is_aligned16(a.ins[q]));
+        if (u < un.total()) v[i] = scale(load_user_unit(a.ins[q], u, un, is_aligned16(a.ins[q])));
       }
     }
 #pragma unroll
@@ -105,6 +114,14 @@ __global__ void __launch_bounds__(kThreads, 1) reducescatterv_kernel(DevComm c, 
   }
   finish_launch(c);
 }
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reducescatterv_kernel(DevComm c, RSVArgs a) {
+  reducescatterv_body<T, OP>(c, a, NoScale{});
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reducescatterv_kernel(DevComm c, RSVArgs a, PremulArg f) {
+  reducescatterv_body<T, OP>(c, a, Premul<T>(f));
+}
 
 // One window [u0, u0 + units) of a table's packed stream of output units; n sub-slots of
 // units * 16 bytes fit one staging slot.
@@ -117,16 +134,25 @@ struct RSTableArgs {
 };
 static_assert(fits_param_space<RSTableArgs>(), "reduce-scatter table exceeds the kernel parameter space");
 
-template <typename T, int OP>
-__global__ void __launch_bounds__(kThreads, 1)
-    reducescatter_table_kernel(DevComm c, const __grid_constant__ RSTableArgs a) {
+template <typename T, int OP, typename S>
+__device__ __forceinline__ void reducescatter_table_body(const DevComm &c, const RSTableArgs &a, const S &scale) {
   reducescatter_push_body(
       c, a.staging_bytes, a.units,
       [&](size_t u) {
         const int k = table_entry(a.t.ustart, a.t.count, a.u0 + u);
-        return PeerParts<const char *>{a.ins[k], a.u0 + u - a.t.ustart[k], make_units(a.t.nbytes[k])};
+        return scaled(PeerParts<const char *>{a.ins[k], a.u0 + u - a.t.ustart[k], make_units(a.t.nbytes[k])}, scale);
       },
       [&](size_t u, const uint4(&v)[kMaxRanks], int n) { table_store_unit(a.t, a.u0 + u, reduce_ranks<T, OP>(v, n)); });
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1)
+    reducescatter_table_kernel(DevComm c, const __grid_constant__ RSTableArgs a) {
+  reducescatter_table_body<T, OP>(c, a, NoScale{});
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1)
+    reducescatter_table_kernel(DevComm c, const __grid_constant__ RSTableArgs a, PremulArg f) {
+  reducescatter_table_body<T, OP>(c, a, Premul<T>(f));
 }
 
 struct ReduceArgs {
@@ -137,8 +163,8 @@ struct ReduceArgs {
 };
 
 // Every rank stages its tensor; the root pulls all n copies and reduces in place.
-template <typename T, int OP>
-__global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceArgs a) {
+template <typename T, int OP, typename S>
+__device__ __forceinline__ void reduce_body(const DevComm &c, const ReduceArgs &a, const S &scale) {
   const uint32_t launch = c.st->launch_ctr;
   const uint32_t ep = launch * 4u;
   const int n = c.world, r = c.rank;
@@ -150,7 +176,7 @@ __global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceAr
   const size_t first = size_t(blockIdx.x) * kThreads + threadIdx.x;
 
   char *mine = c.data[r] + off;
-  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), load_user_unit(a.buf, u, un, al));
+  for (size_t u = first; u < U; u += stride) st_vec(mine + (u << 4), scale(load_user_unit(a.buf, u, un, al)));
 
   if (!cta_barrier_all(c, ep + 1)) {
     finish_launch(c);
@@ -168,9 +194,17 @@ __global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceAr
   }
   finish_launch(c);
 }
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceArgs a) {
+  reduce_body<T, OP>(c, a, NoScale{});
+}
+template <typename T, int OP>
+__global__ void __launch_bounds__(kThreads, 1) reduce_kernel(DevComm c, ReduceArgs a, PremulArg f) {
+  reduce_body<T, OP>(c, a, Premul<T>(f));
+}
 
 // a kernel of this file's CUDA module, for preload_kernels() (bootstrap.cu)
-const void *reduce_ops_module_anchor() { return reinterpret_cast<const void *>(&reducescatter_kernel<float, B200_SUM>); }
+const void *reduce_ops_module_anchor() { return reinterpret_cast<const void *>(static_cast<void (*)(DevComm, RSArgs)>(&reducescatter_kernel<float, B200_SUM>)); }
 
 }  // namespace b200
 
@@ -180,7 +214,8 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
                                   int dtype, int op, void *stream_) {
   int rc;
   size_t es;
-  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op))) return rc;
+  OpArg oa;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(c, op, dtype, &oa))) return rc;
   if (count == 0) return B200_OK;
   if (!ins || !out) return null_tensor_error();
   for (int p = 0; p < c->world; ++p)
@@ -192,6 +227,7 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   const size_t total = count * es;
   if (c->world == 1) {
+    if (oa.op == kOpPremulSum) return launch_premul_scale(c, ins[0], out, total, dtype, oa.premul, stream);
     if (ins[0] != out) B200_CHECK_CUDA(cudaMemcpyAsync(out, ins[0], total, cudaMemcpyDeviceToDevice, stream));
     return B200_OK;
   }
@@ -203,6 +239,11 @@ extern "C" int b200_reducescatter(b200_comm_t c, const void *const *ins, void *o
     a.out = static_cast<char *>(out) + done;
     a.nbytes = nbytes;
     a.staging_bytes = c->staging_bytes;
+    if (oa.op == kOpPremulSum)
+      B200_DISPATCH_PREMUL(dtype, T, {
+        return launch_staged(c, reducescatter_kernel<T, kOpPremulSum>, a, make_units(nbytes).total(), stream,
+                             oa.premul);
+      });
     B200_DISPATCH_DTYPE(dtype, T,
                         B200_DISPATCH_OP(op, OP, { return launch_staged(c, reducescatter_kernel<T, OP>, a,
                                                                         make_units(nbytes).total(), stream); }));
@@ -213,7 +254,8 @@ extern "C" int b200_reducescatterv(b200_comm_t c, const void *const *ins, const 
                                    int dtype, int op, void *stream_) {
   int rc;
   size_t es;
-  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op)) ||
+  OpArg oa;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(c, op, dtype, &oa)) ||
       (rc = check_list(c->world, ins && counts)))
     return rc;
   const int n = c->world;
@@ -227,7 +269,9 @@ extern "C" int b200_reducescatterv(b200_comm_t c, const void *const *ins, const 
   if (nbytes[c->rank] && !out) return null_tensor_error();
   if (even) return b200_reducescatter(c, ins, out, counts[0], dtype, op, stream_);  // also world 1
   void (*kernel)(DevComm, RSVArgs) = nullptr;
-  B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatterv_kernel<T, OP>; }));
+  void (*premul_kernel)(DevComm, RSVArgs, PremulArg) = nullptr;
+  if (oa.op == kOpPremulSum) B200_DISPATCH_PREMUL(dtype, T, { premul_kernel = reducescatterv_kernel<T, kOpPremulSum>; })
+  else B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatterv_kernel<T, OP>; }));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   RSVArgs a{};
@@ -241,7 +285,8 @@ extern "C" int b200_reducescatterv(b200_comm_t c, const void *const *ins, const 
     }
     a.out = a.nbytes[c->rank] ? static_cast<char *>(out) + (u0 << 4) : nullptr;
     a.units = units;
-    return launch_staged(c, kernel, a, units, stream);
+    return premul_kernel ? launch_staged(c, premul_kernel, a, units, stream, oa.premul)
+                         : launch_staged(c, kernel, a, units, stream);
   });
 }
 
@@ -249,7 +294,8 @@ extern "C" int b200_reducescatter_multi(b200_comm_t c, const void *const *ins, v
                                         const size_t *counts, int ntensors, int dtype, int op, void *stream_) {
   int rc;
   size_t es;
-  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op)) ||
+  OpArg oa;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(c, op, dtype, &oa)) ||
       (rc = check_list(ntensors, ins && outs && counts)))
     return rc;
   std::vector<size_t> nbytes(static_cast<size_t>(ntensors));
@@ -261,9 +307,17 @@ extern "C" int b200_reducescatter_multi(b200_comm_t c, const void *const *ins, v
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   const int n = c->world;
+  if (n == 1 && oa.op == kOpPremulSum) {
+    for (int i = 0; i < ntensors; ++i)
+      if ((rc = launch_premul_scale(c, ins[i], outs[i], nbytes[i], dtype, oa.premul, stream))) return rc;
+    return B200_OK;
+  }
   if (n == 1) return copy_list_local(outs, ins, nbytes.data(), ntensors, stream);
   void (*kernel)(DevComm, const RSTableArgs) = nullptr;
-  B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatter_table_kernel<T, OP>; }));
+  void (*premul_kernel)(DevComm, const RSTableArgs, PremulArg) = nullptr;
+  if (oa.op == kOpPremulSum)
+    B200_DISPATCH_PREMUL(dtype, T, { premul_kernel = reducescatter_table_kernel<T, kOpPremulSum>; })
+  else B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, { kernel = reducescatter_table_kernel<T, OP>; }));
   // One launch per window of each table's stream of output units; the n sub-slots of a window
   // fill at most one staging slot.
   RSTableArgs a{};
@@ -276,7 +330,8 @@ extern "C" int b200_reducescatter_multi(b200_comm_t c, const void *const *ins, v
       [&](size_t done, size_t units) -> int {
         a.u0 = done;
         a.units = units;
-        return launch_staged(c, kernel, a, units, stream);
+        return premul_kernel ? launch_staged(c, premul_kernel, a, units, stream, oa.premul)
+                             : launch_staged(c, kernel, a, units, stream);
       });
 }
 
@@ -284,16 +339,22 @@ extern "C" int b200_reduce(b200_comm_t c, void *buf, size_t count, int dtype, in
                            void *stream_) {
   int rc;
   size_t es;
-  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(op)) ||
+  OpArg oa;
+  if ((rc = check_usable(c)) || (rc = check_dtype(dtype, &es)) || (rc = check_op(c, op, dtype, &oa)) ||
       (rc = check_rank(c, root, "root")))
     return rc;
   if (count == 0) return B200_OK;
   if (!buf) return null_tensor_error();
-  if (c->world == 1) return B200_OK;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (c->world == 1)
+    return oa.op == kOpPremulSum ? launch_premul_scale(c, buf, buf, count * es, dtype, oa.premul, stream) : B200_OK;
   B200_CHECK_CUDA(cudaSetDevice(c->device));
   return for_each_piece(count * es, c->staging_bytes, [&](size_t done, size_t nbytes) -> int {
     const ReduceArgs a{static_cast<char *>(buf) + done, nbytes, c->staging_bytes, root};
+    if (oa.op == kOpPremulSum)
+      B200_DISPATCH_PREMUL(dtype, T, {
+        return launch_staged(c, reduce_kernel<T, kOpPremulSum>, a, make_units(nbytes).total(), stream, oa.premul);
+      });
     B200_DISPATCH_DTYPE(dtype, T, B200_DISPATCH_OP(op, OP, {
                           return launch_staged(c, reduce_kernel<T, OP>, a, make_units(nbytes).total(), stream);
                         }));

@@ -28,6 +28,23 @@ struct PeerParts {
   }
 };
 
+// A unit source whose loads are scaled (PREMUL_SUM's reduce-scatter sources); scaled() leaves a
+// source as it is under NoScale, so the plain kernels pass the body exactly what they did before.
+template <typename Src, typename S>
+struct ScaledParts {
+  Src src;
+  S scale;
+  __device__ __forceinline__ uint4 load(int q) const { return scale(src.load(q)); }
+};
+template <typename Src>
+__device__ __forceinline__ Src scaled(const Src &src, const NoScale &) {
+  return src;
+}
+template <typename Src, typename T>
+__device__ __forceinline__ ScaledParts<Src, Premul<T>> scaled(const Src &src, const Premul<T> &s) {
+  return {src, s};
+}
+
 // All-gather: stage units [0, mine_units) of this rank's part, load(u) each, in the own slot; after
 // the barrier every unit u of [0, units) with at(u).has(p) is pulled from rank p's slot, and
 // at(u).store(p, v) stores it (and stores nothing where rank p's part lacks unit u).  The peer
@@ -169,6 +186,15 @@ inline int launch_staged(b200_comm *c, void (*kernel)(DevComm, Args), const Args
                          cudaStream_t stream) {
   const int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
   kernel<<<g, kThreads, 0, stream>>>(c->dev(), a);
+  B200_LAUNCH_CHECK(c);
+  return B200_OK;
+}
+// ... and a PREMUL_SUM kernel, which takes the factor as one more argument
+template <typename Args>
+inline int launch_staged(b200_comm *c, void (*kernel)(DevComm, Args, PremulArg), const Args &a, size_t units,
+                         cudaStream_t stream, const PremulArg &f) {
+  const int g = pick_blocks(c, (units + kThreads - 1) / kThreads, c->sm_count);
+  kernel<<<g, kThreads, 0, stream>>>(c->dev(), a, f);
   B200_LAUNCH_CHECK(c);
   return B200_OK;
 }

@@ -24,7 +24,7 @@ import torch
 import torch.distributed as dist
 
 from .. import _native as N
-from ..comm import B200Comm
+from ..comm import B200Comm, PremulSum
 from ..store import TorchDistStore
 
 BACKEND_NAME = "b200"
@@ -33,7 +33,11 @@ _group_counter = 0
 _counter_lock = threading.Lock()
 
 
-def _op_code(reduce_op) -> int:
+def _op_code(reduce_op):
+    """The B200Comm op of a c10d ReduceOp: an ``N.*`` code, or a ``PremulSum`` carrying the factor of
+    ``dist._make_nccl_premul_sum(factor)`` (a float or a one-element tensor)."""
+    if reduce_op == dist.ReduceOp.PREMUL_SUM:
+        return PremulSum(reduce_op.__getstate__()[1])
     table = ((dist.ReduceOp.SUM, N.SUM), (dist.ReduceOp.PRODUCT, N.PROD), (dist.ReduceOp.MIN, N.MIN),
              (dist.ReduceOp.MAX, N.MAX), (dist.ReduceOp.AVG, N.AVG))
     for torch_op, code in table:
@@ -230,6 +234,14 @@ class B200ProcessGroup(dist.ProcessGroup):
                                                    self._rank, self._size, self._timeout)
             return self._gloo
 
+    @staticmethod
+    def _with_factor(tensors, op):
+        """``tensors`` plus a ``PremulSum`` op's CUDA factor, which the kernels read on the
+        communication stream and ``_run`` therefore records there; ``tensors`` itself otherwise."""
+        if isinstance(op, PremulSum) and op.device_factor is not None:
+            return list(tensors) + [op.device_factor]
+        return tensors
+
     def _run(self, tensors: List[torch.Tensor], fn, result, tag: str = "op") -> B200Work:
         """Enqueue ``fn(comm)`` on the communication stream, ordered after the caller's stream."""
         dev = tensors[0].device
@@ -272,13 +284,14 @@ class B200ProcessGroup(dist.ProcessGroup):
             for t in tensors:
                 comm.allreduce(self._contig(t), op)
 
-        return self._run(tensors, fn, tensors)
+        return self._run(self._with_factor(tensors, op), fn, tensors)
 
     def allreduce_coalesced(self, tensors, opts=None):
         if not self._all_cuda(tensors):
             return self._cpu_group().allreduce_coalesced(tensors, opts)
         op = _op_code(opts.reduceOp) if opts is not None else N.SUM
-        return self._run(tensors, lambda comm: comm.allreduce_multi([self._contig(t) for t in tensors], op), tensors)
+        return self._run(self._with_factor(tensors, op),
+                         lambda comm: comm.allreduce_multi([self._contig(t) for t in tensors], op), tensors)
 
     def broadcast(self, tensors, opts=None):
         if not self._all_cuda(tensors):
@@ -415,7 +428,7 @@ class B200ProcessGroup(dist.ProcessGroup):
                                              [[self._contig(i) for i in lst] for lst in ins], op)
 
             flat = list(output_tensors) + [i for ins in input_tensors for i in ins]
-            return self._run(flat, fn_multi, output_tensors)
+            return self._run(self._with_factor(flat, op), fn_multi, output_tensors)
 
         def fn(comm):
             for out, ins in zip(output_tensors, input_tensors):
@@ -427,11 +440,11 @@ class B200ProcessGroup(dist.ProcessGroup):
                     comm.reducescatter(self._contig(out), [self._contig(i) for i in ins], op)
 
         flat = list(output_tensors) + [i for ins in input_tensors for i in ins]
-        return self._run(flat, fn, output_tensors)
+        return self._run(self._with_factor(flat, op), fn, output_tensors)
 
     def _reduce_scatter_base(self, output, input, opts=None):  # noqa: A002
         op = _op_code(opts.reduceOp) if opts is not None else N.SUM
-        return self._run([output, input],
+        return self._run(self._with_factor([output, input], op),
                          lambda comm: comm.reducescatter_from(self._contig(output), self._contig(input), op), output)
 
     def reduce_scatter_tensor_coalesced(self, outputs, inputs, opts=None):
@@ -448,7 +461,7 @@ class B200ProcessGroup(dist.ProcessGroup):
             for outs, ins in self._by_dtype(outputs, inputs):
                 comm.reducescatter_from_multi([self._contig(o) for o in outs], [self._contig(i) for i in ins], op)
 
-        return self._run(list(outputs) + list(inputs), fn, outputs)
+        return self._run(self._with_factor(list(outputs) + list(inputs), op), fn, outputs)
 
     def reduce(self, tensors, opts=None):
         if not self._all_cuda(tensors):
@@ -460,7 +473,7 @@ class B200ProcessGroup(dist.ProcessGroup):
             for t in tensors:
                 comm.reduce(self._contig(t), root, op)
 
-        return self._run(tensors, fn, tensors)
+        return self._run(self._with_factor(tensors, op), fn, tensors)
 
     def barrier(self, opts=None):
         if self._comm is None or not torch.cuda.is_available():
